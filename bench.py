@@ -60,11 +60,48 @@ def parse():
     ap.add_argument('--workload', default='c2', choices=sorted(WORKLOADS))
     ap.add_argument('--inflight', type=int, default=3,
                     help='scans in flight per GPU in the timed legs (harness.ScanPipeline); 1 = strictly one after another')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last device-resident step computed as DIR/<name>.npy '
+                         '(float32 / float64, at most 64 MB in all) so that two builds can be compared output for output')
     return ap.parse_args()
 
 
+DUMP_BUDGET = 64 << 20
+
+
+def dump_outputs(ret, out_dir, seed=0):
+    """Every tensor of the forward's result dict (nested dicts flattened as parent.child) -> out_dir/<name>.npy: floating
+    values as float32, integer / boolean ones as float64 (exact below 2^53). An array whose share of the 64 MB budget is
+    exceeded is replaced by a fixed, seeded sample of its rows (sorted row indices, the same for the same row count); the
+    row indices are written beside it as <name>.rows.npy."""
+    import torch
+    arrays = {}
+
+    def walk(prefix, v):
+        if isinstance(v, dict):
+            for k in sorted(v):
+                walk(prefix + '.' + str(k) if prefix else str(k), v[k])
+        elif isinstance(v, torch.Tensor):
+            arrays[prefix] = v.detach().cpu().numpy()
+        elif isinstance(v, np.ndarray):
+            arrays[prefix] = v
+
+    walk('', ret)
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BUDGET // max(1, 2 * len(arrays))  # half the budget per array share: room for the sampled row indices
+    for name, a in sorted(arrays.items()):
+        a = a.astype(np.float32) if np.issubdtype(a.dtype, np.floating) else a.astype(np.float64)
+        if a.nbytes > share and a.ndim >= 1 and a.shape[0] > 0:
+            row_bytes = a.nbytes // a.shape[0]
+            k = max(1, share // max(row_bytes, 1))
+            rows = np.sort(np.random.RandomState(seed).choice(a.shape[0], size=min(k, a.shape[0]), replace=False))
+            a = a[rows]
+            np.save(os.path.join(out_dir, name + '.rows.npy'), rows.astype(np.float64))
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+
+
 # ---------------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md "clocks DURING the timed region")
+# clocks sampling during the timed region (read-only nvidia-smi queries)
 # ---------------------------------------------------------------------------------------------------------
 class ClockSampler(object):
     Q = ('clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,'
@@ -239,11 +276,11 @@ def cpu_leg(args, sd, cfg, scan, steps, warmup):
 
 
 def reference_gpu_ops_leg(scan, cfg, inj, out, reps=3):
-    """The reference's OWN CUDA/CPU ops (oracle/_ref: the unmodified softgroup/ops/src compiled for sm_100a) timed on this
-    B200 on the tensors of the same scan, called the way softgroup/ops/functions.py and softgroup/model/softgroup.py call
+    """The reference's OWN CUDA/CPU ops (oracle/_ref: the unmodified softgroup/ops/src compiled for sm_90a) timed on this
+    GPU on the tensors of the same scan, called the way softgroup/ops/functions.py and softgroup/model/softgroup.py call
     them (per-class loop, relaunch when the index buffer overflows, lists copied to the host for the CPU BFS). CUDA events
     around each call sequence; median of `reps`. Reported beside `roofline.by_kernel` -- a like-for-like kernel baseline,
-    not a target. Returns None when oracle/_ref is not on the box."""
+    not a target. Returns None when oracle/_ref has not been built."""
     import torch
     from oracle.build_ref import load_ref
     try:
@@ -358,7 +395,7 @@ def reference_gpu_ops_leg(scan, cfg, inj, out, reps=3):
 
         _, (ms, wall) = timed(gap)
         res['global_avg_pool_fp'] = dict(ms=ms, wall_ms=wall, rows=int(pidx.size(0)))
-    res['note'] = ('unmodified reference ops (oracle/_ref, sm_100a build) on this B200, same scan and injected predictions; '
+    res['note'] = ('unmodified reference ops (oracle/_ref, sm_90a build) on this GPU, same scan and injected predictions; '
                    'spconv (third party) is not part of the reference tree and has no entry here')
     return res
 
@@ -416,8 +453,8 @@ def main():
     assert torch.cuda.is_available(), 'bench.py needs a GPU (no CPU fallback)'
     torch.cuda.set_device(local_rank)
     # The host side of a scan is launch latency, not throughput: no intra-op pool and, with one rank per GPU, every rank on its
-    # own share of the cores of ITS GPU's NUMA node (NVML's ideal CPU affinity; the GPUs of the 8-GPU box sit four per node).
-    torch.set_num_threads(1)  # (1 / 8 / 128 threads measured the same on one GPU: GPU call 33; 1 keeps 8 ranks x 3 scan threads quiet)
+    # own share of the cores of ITS GPU's NUMA node (NVML's ideal CPU affinity; multi-GPU machines put several GPUs on a node).
+    torch.set_num_threads(1)  # (the intra-op pool does not help a launch-bound host side; 1 keeps 8 ranks x 3 scan threads quiet)
     if world > 1:
         try:
             import pynvml
@@ -460,7 +497,7 @@ def main():
                                       confusion=wl.get('confusion', 0.0))
     dev = harness.device_batch(hb)
     dev_in = {k: v for k, v in dev.items() if k not in ('voxel_coords', 'v2p_map', 'p2v_map')}
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')  # 2x the 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')  # 5x the 50 MB L2 of an H100
 
     def step_device():
         # inputs resident in HBM; the step includes the GPU hash (point->voxel) and the whole forward
@@ -481,10 +518,10 @@ def main():
             out = None
             for _ in range(warmup):
                 out = fn()  # (kept while the next call runs, like in the timed loop: the second set of pinned result buffers
-                            #  is then allocated here and not by a 25 ms cudaHostAlloc inside the second timed step)
+                            #  is then allocated here and not by a cudaHostAlloc inside the second timed step)
             # every object alive after the warm-up (model, plans, cached tensors) moves to the permanent generation: a full
-            # collection of Python's cyclic GC in the middle of a timed step cost 10-20 ms once per leg (one 23-31 ms step
-            # among 20 of 10.9 ms end to end, GPU call 40)
+            # collection of Python's cyclic GC in the middle of a timed step stalls every scan thread and shows up as one
+            # outlier step per leg
             gc.collect()
             gc.freeze()
             barrier()
@@ -539,6 +576,8 @@ def main():
         seq_dev_ms, dev_wall, out = timed(step_device, args.steps, max(args.warmup, 3))
         launches = (_lib.lib().sgb_launch_count() - l0)
         seq_dev_steps = sorted(timed.last_per_step)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(out, args.dump_outputs, seed=args.seed)
         seq_e2e_ms, e2e_wall, ret = timed(lambda: harness.run_scan(model, hb, inject_pointwise=inj), args.steps, 3)
         seq_e2e_steps = sorted(timed.last_per_step)
         if pipe is not None:
@@ -576,29 +615,14 @@ def main():
             peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
         except Exception:
             pass
-        hbm_peak = float(peaks.get('hbm_gbs', 6650.0))
-        peak_src = 'measured (MEASURED_PEAKS.json)' if 'hbm_gbs' in peaks else 'fallback (B200_PROFILING.md)'
+        hbm_peak = float(peaks.get('hbm_gbs', 3350.0))
+        peak_src = 'measured (MEASURED_PEAKS.json)' if 'hbm_gbs' in peaks else 'H100 SXM data sheet (HBM3, 3.35 TB/s)'
         prof = profiler.summary()
         dom = prof['dominant']
         traffic = None
         traffic_note = None
-        try:  # dram__bytes_read+write of the conv launches from the committed OFFLINE ncu capture (per step, like achieved)
-            tj = json.load(open(os.path.join(ROOT, 'profiles', 'r2_dominant_kernel_traffic.json')))
-            if tj.get('kernel') == dom['name'] and args.workload == 'c2':
-                traffic = tj['dram_bytes_per_step']
-                traffic_note = tj.get('note')
-        except Exception:
-            pass
         for k, v in prof['by_kernel'].items():
             v['frac_of_hbm_peak'] = round(v['gbs'] / hbm_peak, 4)
-        if args.workload == 'c2' and 'ballquery_batch_p' in prof['by_kernel']:
-            # the ball query is bound by instruction issue, not bytes (DESIGN.md 6): its floor from the committed ncu capture
-            # (8.2 M warp-level blocks of 32 exact distance tests per scan at >= 9 thread-instructions per test on 148 SMs x 128
-            # lanes at 1.965 GHz ~ 63 us; 416 M warp instructions executed at 57 % issue-slot utilisation)
-            bq = prof['by_kernel']['ballquery_batch_p']
-            bq['issue_floor_us'] = 63.0
-            bq['frac_of_issue_floor'] = round(63.0 / max(bq['ms_per_step'] * 1e3, 1e-9), 4)
-            bq['issue_floor_source'] = 'offline: profiles/r2_ncu_grouping_per_launch.tsv + the instruction count of the test loop'
         roofline = dict(bound='hbm', kernel=dom['name'], achieved=dom['gbs'], peak=hbm_peak, unit='GB/s',
                         frac=dom['gbs'] / hbm_peak, traffic=traffic, traffic_source=traffic_note, peak_source=peak_src,
                         launches_per_step=dom['launches_per_step'], avg_launch_us=dom['avg_us'],
@@ -616,7 +640,7 @@ def main():
                                 'outputs are computed, then overwritten by synthetic predictions (one-hot*8+N(0,1), centroid '
                                 'offsets+N(0,sigma)) so grouping sees a trained-checkpoint load' %
                                 (wl['cfg'], cfg['channels'], cfg['num_blocks']),
-                                l2='flushed: 256 MiB memset (2x the L2) before every scan (between the per-step events of the sequential legs; inside the timed '
+                                l2='flushed: 256 MiB memset (more than 2x the L2) before every scan (between the per-step events of the sequential legs; inside the timed '
                                 'region, on the scan\'s own stream, with scans in flight)',
                                 parallelism='dp%d (independent scans, no data-path collective)' % world,
                                 inflight='%d scans in flight per GPU (host thread + CUDA stream each); one at a time: see '

@@ -1,5 +1,5 @@
 /*
- * sgb200.h -- C ABI of libsgb200.so, the B200 (sm_100a) implementation of SoftGroup's per-scan
+ * sgb200.h -- C ABI of libsgb200.so, the H100 (sm_90a) implementation of SoftGroup's per-scan
  * inference hot path (reference: thangvubk/SoftGroup, paths below are relative to its root).
  *
  * Boundary rules
@@ -204,7 +204,7 @@ int sgb_spconv_forward(const float *d_in, int in_stride, int in_off, const int32
                        int out_stride, int out_off, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Tensor-core sparse convolution (spconv_tc.cu; tcgen05.mma kind::f16, fp32 accumulators in TMEM) -- the production path
+ * Tensor-core sparse convolution (spconv_tc.cu; wgmma.mma_async f16, fp32 accumulators in registers) -- the production path
  * for Cin <= 512, Cout <= 256. Every operand value x is carried as two fp16 numbers hi = fp16(x),
  * lo = fp16((x - hi) * 2^shift), shift = sgb_spconv_lo_shift(), and the product is hi*hi + hi*lo + lo*hi: fp32-grade
  * (DESIGN.md 3.2). Activations travel PACKED between convolutions: per row and 32-channel chunk 16 words of fp16 hi pairs
@@ -212,7 +212,7 @@ int sgb_spconv_forward(const float *d_in, int in_stride, int in_off, const int32
  *   Weights, pre-split and pre-packed by the host (softgroup_b200/spconv/core.py:pack_weight_tc) with the same shift:
  *     N = Cout rounded up to 16, nkc = ceil(Cin/32);
  *     Wp fp16 [K][nkc][4][2][N][8]: element (k, kc, q, part, n, e) = part(W[k][32*kc + 8*q + e][n]) (0 outside Cin/Cout),
- *     part 0 = hi, part 1 = lo -- per (k, kc) a UMMA K-major / no-swizzle operand [B_hi | B_lo] of 16-byte chunks;
+ *     part 0 = hi, part 1 = lo -- per (k, kc) the K-major / no-swizzle wgmma B operands B_hi, B_lo of 16-byte chunks;
  *     passed as float* (two halves per word); sgb_spconv_tc_packed_floats = its length in words.
  *   sgb_spconv_forward_tc: d_in_pk packed input [Min][in_stride words] ALREADY activated (the consumer's
  *     BatchNorm(eval)+ReLU was applied by whoever packed it); d_map int32 [K][Mout] (-1 = no neighbour) or NULL for the
@@ -223,8 +223,8 @@ int sgb_spconv_forward(const float *d_in, int in_stride, int in_off, const int32
  *   sgb_act_pack: the same packing for tensors without a producing convolution (C real channels, zeros up to Cfill).
  *   sgb_spconv_overflow: a packed value beyond the fp16 range (|y| > 65504, or NaN) raises a per-device flag instead of
  *     saturating silently; this call reads and clears it (blocking 4-byte read on `stream`).
- *   sgb_spconv_tc_plan: the tile configuration the launch uses for a problem size (pure function; sms <= 0: 148):
- *     out[0] = NT (columns per CTA), [1] = column parts, [2] = split-K cluster size, [3] = TMEM columns per CTA,
+ *   sgb_spconv_tc_plan: the tile configuration the launch uses for a problem size (pure function; sms <= 0: 132):
+ *     out[0] = NT (columns per CTA), [1] = column parts, [2] = split-K cluster size, [3] = shared memory per CTA (bytes),
  *     [4] = pipeline stages, [5] = row tiles.
  * ------------------------------------------------------------------------------------------- */
 long long sgb_spconv_tc_packed_floats(int K, int Cin, int Cout);
@@ -238,12 +238,12 @@ int sgb_spconv_forward_tc(const float *d_in_pk, int in_stride, int Min, const in
                           const float *d_bias, float *d_out, int out_stride, int out_off, float *d_pk_out, int pk_stride,
                           int pk_coff, const float *d_pk_scale, const float *d_pk_shift, int pk_relu, int pk_fill,
                           void *stream);
-/* Two kernels implement sgb_spconv_forward_tc with bit-identical results (same products, same accumulation order):
- *   0 = register gather (spconv_tc.cu: rows -> registers -> tensor memory, column split and split-K clusters for the deep
- *       U-Net levels), 1 = persistent shared-memory ring (spconv_ss.cu: cp.async row gather into SWIZZLE_128B tiles, one
- *       CTA per SM walking the row tiles, accumulators double-buffered in tensor memory).
- * sgb_spconv_kernel_choice: which one sgb_spconv_forward_tc runs for a problem size (sms <= 0: 148).
- * sgb_spconv_forward_tc_ex: the same call with the kernel named explicitly (-1 = choose) -- parity tests and A/B tools. */
+/* Two launch forms of one kernel implement sgb_spconv_forward_tc with bit-identical results (same products, same
+ * accumulation order; split-K sums partial tiles in rank order):
+ *   0 = one CTA per work item (128 rows x NT columns), column split and split-K thread-block clusters for the deep
+ *       U-Net levels, 1 = persistent (as many CTAs as fit on the GPU walk the work items).
+ * sgb_spconv_kernel_choice: which form sgb_spconv_forward_tc runs for a problem size (sms <= 0: 132).
+ * sgb_spconv_forward_tc_ex: the same call with the form named explicitly (-1 = choose) -- parity tests and A/B tools. */
 int sgb_spconv_kernel_choice(int K, int Mout, int Cin, int Cout, int sms);
 int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const int32_t *d_map, int K, int Mout,
                              const float *d_Wp, int Cin, int Cout, const float *d_residual, int res_stride, int res_off,

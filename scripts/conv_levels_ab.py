@@ -1,4 +1,4 @@
-"""Per-level timing of one SubM 3x3x3 convolution (C_l -> C_l) on the rulebooks of the 150k-point bench scan (tcgen05
+"""Per-level timing of one SubM 3x3x3 convolution (C_l -> C_l) on the rulebooks of the 150k-point bench scan (tensor-core
 kernel; --morton puts the rows in Z-order first). L2 is flushed before every timed launch; the packed
 input is prepared outside the timed region so the number is the conv kernel alone.
 Usage: python scripts/conv_levels_ab.py [impl ...]"""

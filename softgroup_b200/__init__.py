@@ -1,4 +1,4 @@
-"""softgroup_b200 -- B200 (sm_100a) implementation of SoftGroup's per-scan inference hot path.
+"""softgroup_b200 -- H100 (sm_90a) implementation of SoftGroup's per-scan inference hot path.
 
 Layout: csrc/ (CUDA kernels + C ABI, built into libsgb200.so), ops/ (the reference's softgroup.ops binding
 surface), spconv/ (the spconv-shaped surface the reference model touches), model/ (SoftGroup nn.Module mirror),

@@ -1,6 +1,6 @@
-"""Compile softgroup_b200/csrc/*.cu into softgroup_b200/libsgb200.so (sm_100a only, in-tree).
+"""Compile softgroup_b200/csrc/*.cu into softgroup_b200/libsgb200.so (sm_90a only, in-tree).
 
-nvcc cross-compiles without a GPU. The .so is git-ignored but travels to the GPU box with the snapshot.
+nvcc cross-compiles without a GPU. The .so and the objects under csrc/build/ are build products (git-ignored).
 """
 import glob
 import os
@@ -14,7 +14,7 @@ OBJ = os.path.join(HERE, 'csrc', 'build')
 LIB = os.path.join(HERE, 'libsgb200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+    '-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
     '--expt-relaxed-constexpr'
 ]
 
@@ -46,7 +46,7 @@ def build(force=False, verbose=False):
             list(ex.map(run, jobs))
     objs = [os.path.join(OBJ, os.path.basename(s)[:-3] + '.o') for s in srcs]
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a', '-cudart', 'static']
+        cmd = [NVCC, '-shared', '-o', LIB] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a', '-cudart', 'static']
         if verbose:
             print(' '.join(cmd), file=sys.stderr)
         subprocess.check_call(cmd)

@@ -24,14 +24,14 @@
 
 namespace sgb {
 
-// Two 512-thread CTAs per SM (round 2; round 1 ran one 1024-thread CTA with a 160 KB staging area): the CTA-wide
-// barriers of the staging / ordering phases were 39 % of the stall samples (profiles/r1_ncu_bq_summary.txt) -- with two
-// CTAs one stages while the other queries, and each barrier spans half as many warps.
+// Two 512-thread CTAs per SM (round 1 ran one 1024-thread CTA with a 160 KB staging area): the CTA-wide barriers of the
+// staging / ordering phases were the largest stall reason -- with two CTAs one stages while the other queries, and each
+// barrier spans half as many warps.
 // Pass 0 of the query: 512-thread CTAs, two per SM, 5120 staged candidates (80 KB) each. Work items whose stencil is
 // larger (the core cells of collapsed objects: several thousand candidates) are only NOTED in pass 0 and processed by
-// pass 1: one 1024-thread CTA per SM with a 10240-candidate staging area (the round-1 configuration). Measured (GPU
-// calls 6/7 of round 2): the small configuration alone is 1.7x faster on fragmented predictions (2.34 -> 1.37 ms) but
-// 1.4x slower on the clean 40-object scan (1.35 -> 1.89 ms, its cores overflow into the exact-scan path).
+// pass 1: one 1024-thread CTA per SM with a 10240-candidate staging area (the round-1 configuration). The small
+// configuration alone is faster on fragmented predictions but slower on the clean 40-object scan, whose cores overflow
+// into the exact-scan path.
 template <int PASS> struct BqCfg;
 template <> struct BqCfg<0> { static constexpr int kThreads = 512, kSMax = 5120, kBmWords = 4096, kPerSM = 2; };
 template <> struct BqCfg<1> { static constexpr int kThreads = 1024, kSMax = 10240, kBmWords = 8192, kPerSM = 1; };
@@ -327,7 +327,7 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
       }
       }  // !ordered
       // ---- queries of this cell: one warp each ----------------------------------------------------
-      // The two loops below are 78 % of the kernel's 607 M warp instructions (ncu source page, round 2): they run on raw
+      // The two loops below are most of the kernel's instructions: they run on raw
       // 32-bit shared-memory addresses (the generic-pointer form re-derived the shared window base in every iteration) and
       // without a bounds test -- the staged stencil is padded to a multiple of 32 with records that can never hit (NaN).
       const int total_pad = (total_s + 31) & ~31;

@@ -82,10 +82,10 @@ __device__ __forceinline__ unsigned long long ld_ca_u64(const unsigned long long
 //           pushed last time (`w.wins`, idle until the emit phase, keeps the last pushed label). Such nodes go into a
 //           queue (node, label to push).
 //   push:   one WARP per queue entry pushes the label to every listed node (4 bytes per edge are read once per CHANGE of the
-//           source label instead of once per pass: 1.43 -> 0.86 ms per 150k-point scan, round 2).
-// Until GPU call 35 both steps ran in one kernel with a static node -> warp mapping; passes 2-3 of a 150k-point scan, where
-// 40 % resp. 2 % of the nodes are active, then took 325 + 233 us against 151 us for the pass that reads EVERY list
-// (ncu: long_scoreboard, a few warps with seven 1000-entry lists each while the others idle). Queue entries cost the same
+//           source label instead of once per pass).
+// Both steps once ran in one kernel with a static node -> warp mapping; passes 2-3 of a 150k-point scan, where 40 %
+// resp. 2 % of the nodes are active, then took longer than the pass that reads EVERY list (a few warps with seven
+// 1000-entry lists each while the others idle). Queue entries cost the same
 // (~1000 edges each), so a strided walk over the queue is balanced.
 // The pass in which nobody is selected ends the iteration: then label[v] <= pushed[u] <= label[u] for every edge u->v,
 // the fixed point of the full iteration. Passes are enqueued in batches without a host round trip: pass `it` raises
@@ -208,7 +208,7 @@ __global__ void bfs_members_kernel(int N, const int32_t *__restrict__ cluster_of
     c = w.cid_of[l];
   }
   // one atomic per (warp, cluster): consecutive nodes mostly belong to the same few components, and 131k single adds on
-  // 40 cursor words serialised in L2 (79 us of a 150k-point scan)
+  // 40 cursor words serialised in L2
   const int lane = threadIdx.x & 31;
   const unsigned peers = __match_any_sync(0xffffffffu, c);
   if (c < 0) return;

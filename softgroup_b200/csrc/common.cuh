@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libsgb200 (sm_100a only).
+// common.cuh -- shared device/host helpers for libsgb200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -34,7 +34,7 @@ void count_launch();  // bumps the process-wide kernel-launch counter (sgb_launc
     }                                                                \
   } while (0)
 
-constexpr int kNumSMs = 148;  // B200
+constexpr int kNumSMs = 132;  // H100 SXM (the launch code asks the device where it can)
 
 static inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }

@@ -1,62 +1,57 @@
-// spconv_tc.cu -- sparse convolution on the 5th-generation tensor cores (tcgen05 + TMEM), sm_100a.
+// spconv_tc.cu -- sparse convolution on the Hopper tensor cores (wgmma, fp32 accumulators in registers), sm_90a.
 //
-// One CTA owns a tile of 128 output rows x NT <= 128 output columns (and, with split-K, a contiguous share of the
-// (kernel offset, 32-channel slice) iterations). For every kernel offset with at least one active pair in the tile
-// and every 32-channel slice of Cin:
-//   * the producer threads gather one input row slice each. Inputs are PACKED rows: activated (the consumer's
-//     BatchNorm(eval)+ReLU) and split once by the PRODUCING convolution's epilogue or by sgb_act_pack. A value x is carried
-//     as two fp16 numbers hi = fp16(x), lo = fp16((x - hi) * 2^kLoShift); both go straight into TENSOR MEMORY with
-//     tcgen05.st (A operand from TMEM: lane = row, 16 columns of hi pairs + 16 columns of lo pairs per stage) -- the
-//     shared-memory pipe only carries the weights;
-//   * the pre-packed weight slice (same split, core-matrix order, done once on the host side) is streamed by one
-//     elected lane with TMA bulk copies into a ring of stages; the weights of the whole convolution are pulled
-//     into L2 with cp.async.bulk.prefetch at kernel start because every CTA walks them in the same order (so they
-//     would otherwise always be cold);
-//   * one thread issues the error-compensated products as tcgen05.mma.cta_group::1.kind::f16 (M=128, K=16)
-//         D[:, 0:2nt]  += A_hi * [B_hi | B_lo]      D[:, nt:2nt] += A_lo * B_hi
-//     accumulating fp32 in TMEM, then tcgen05.commit's the stages back to their producers through mbarriers.
-// The epilogue reads the accumulator with tcgen05.ld, sums the two column blocks, adds bias / residual and writes
-// strided fp32 rows (the U-Net concat buffer) and/or the PACKED rows its consumer reads (that consumer's BatchNorm+ReLU
-// folded in: an intermediate with a single consumer never exists in fp32). With split-K (deep U-Net levels: a handful of row tiles, megabytes of
-// weights) the CTAs of one thread-block cluster hold partial tiles; ranks > 0 park theirs in their own shared memory
-// and rank 0 sums them in rank order over distributed shared memory -- deterministic, no workspace, no atomics.
-// Dropping lo*lo leaves a relative error of ~2^-22 per product, i.e. fp32-grade (the north star's 1e-4 over ~40
-// sequential convolutions rules out plain TF32/fp16; see DESIGN.md).
+// One CTA (two warpgroups, 64 output rows each) owns a work item of 128 output rows x NT <= 128 output columns (and,
+// with split-K, a contiguous share of the item's (kernel offset, 32-channel slice) iterations). For every kernel offset
+// with at least one active pair in the tile and every 32-channel slice of Cin:
+//   * all threads gather the tile's input row slices with cp.async (16 B per copy, zero-fill for absent neighbours)
+//     straight into the SWIZZLE_128B K-major tile the MMA reads. Inputs are PACKED rows: activated (the consumer's
+//     BatchNorm(eval)+ReLU) and split once by the PRODUCING convolution's epilogue or by sgb_act_pack. A value x is
+//     carried as two fp16 numbers hi = fp16(x), lo = fp16((x - hi) * 2^kLoShift): one 128-byte line per row and slice
+//     holds 32 hi values then 32 lo values;
+//   * the pre-packed weight slice (same split, core-matrix order, done once on the host side) is copied next to it;
+//     several stages are in flight, so the L2 latency of the gather overlaps the MMAs of the stages before;
+//   * each warpgroup issues the error-compensated products as wgmma.mma_async m64nNTk16 (fp16 in, fp32 accumulate)
+//         main += A_hi * B_hi      corr += A_hi * B_lo      corr += A_lo * B_hi
+//     and the epilogue forms main + corr * 2^-kLoShift, adds bias / residual and writes strided fp32 rows (the U-Net
+//     concat buffer) and/or the PACKED rows its consumer reads (that consumer's BatchNorm+ReLU folded in: an
+//     intermediate with a single consumer never exists in fp32).
+// Two launch forms of the same kernel (bit-identical results without split-K, see sgb_spconv_kernel_choice):
+//   * kernel 0, one CTA per work item. With few row tiles (deep U-Net levels: a handful of tiles, megabytes of weights)
+//     the columns are split and the CTAs of one thread-block cluster share a tile's iterations (split-K); ranks > 0
+//     park their partial tiles in their own shared memory and rank 0 sums them in rank order over distributed shared
+//     memory -- deterministic, no workspace, no atomics;
+//   * kernel 1, persistent: as many CTAs as fit on the GPU at once walk the work items round-robin.
+// Dropping lo*lo leaves a relative error of ~2^-22 per product, i.e. fp32-grade (1e-4 end to end over ~40 sequential
+// convolutions rules out plain TF32/fp16; see DESIGN.md).
 #include <algorithm>
 #include <cstdlib>
 
 #include <cuda_fp16.h>
 
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 
 namespace sgb {
 
-// spconv_ss.cu: persistent shared-memory-ring kernel (large levels)
-bool spconv_ss_plan(int K, int Mout, int Cin, int Cout, int sms, int *out);
-int spconv_ss_launch(const float *d_in_pk, int in_stride, const int32_t *d_map, int K, int Mout, const float *d_Wp, int Cin,
-                     int Cout, const float *d_residual, int res_stride, int res_off, const float *d_bias, float *d_out,
-                     int out_stride, int out_off, float *d_pk_out, int pk_stride, int pk_coff, const float *d_pk_scale,
-                     const float *d_pk_shift, int pk_relu, int pk_fill, int *d_oflow, int sms, bool *attr_set, cudaStream_t stream);
-
 constexpr int TC_ROWS = 128;
-constexpr int TC_KC = 32;  // channels per stage
-constexpr int TC_THREADS = 320;  // 8 producer warps + 1 MMA warp + 1 weight-loader warp
-// The remainder lo = x - fp16(x) is carried as fp16(lo * 2^kLoShift); the correction columns are scaled back by
-// 2^-kLoShift when they are added to the main product. With shift 0 (round 1) lo was a subnormal fp16 for |x| < ~0.1
-// (2^-25 absolute error) and the per-element 1e-4 bar was missed at C = 224 (2.9e-4, GPU call 3 of round 2); 11 keeps
-// lo normal down to |x| = 2^-14 (sgb_spconv_lo_shift() tells the host weight packer).
+constexpr int TC_KC = 32;        // channels per iteration: one 128-byte packed line per row
+constexpr int TC_THREADS = 256;  // two warpgroups
+constexpr int TC_STAGES = 4;     // gather ring depth
+constexpr int TC_A_BYTES = TC_ROWS * 128;  // 16 KB of rows per stage
+// The remainder lo = x - fp16(x) is carried as fp16(lo * 2^kLoShift); the correction products are scaled back by
+// 2^-kLoShift when they are added to the main product. 11 keeps lo a normal fp16 number down to |x| = 2^-14 (with
+// shift 0 the per-element 1e-4 bar was missed at C = 224); sgb_spconv_lo_shift() tells the host weight packer.
 constexpr int kLoShift = 11;
 constexpr float kLoScale = (float)(1 << kLoShift), kLoInv = 1.0f / kLoScale;
-static_assert(kLoShift == 11, "spconv_ss.cu hard-codes the remainder scale 2^11");
-constexpr int BAR_FULL = 0, BAR_FREE = 3, BAR_BFULL = 9;  // per pair stage (<= 3); bars[8] = accumulator done
 
 struct TcArgs {
-  const float *in; int in_stride, in_off;  // packed rows (words)
-  const int32_t *map; int K, Mout;
-  const float *Wp;  // packed fp16 [K][nkc][4 chunks][2 (hi,lo)][N][8 halves]
-  int Cin, N, Cout;        // N = Cout rounded up to 16
-  int NT;                  // columns per CTA (multiple of 16); gridDim.y = ceil(N / NT)
+  const uint32_t *in; int in_stride;     // packed rows [Min][in_stride words]
+  const int32_t *map; int K, Mout;       // map [K][Mout] (nullptr: identity, K == 1)
+  const float *Wp;                       // packed fp16 [K][nkc][4 chunks][2 (hi,lo)][N][8 halves]
+  int Cin, N, Cout;                      // N = Cout rounded up to 16
+  int nparts;                            // column parts of NT (the last may be shorter)
+  int items;                             // row tiles x column parts
+  int ksplit;                            // CTAs per cluster along z sharing one item's iterations (1 = no split)
   const float *residual; int res_stride, res_off;
   const float *bias;
   float *out; int out_stride, out_off;   // optional fp32 rows
@@ -64,427 +59,237 @@ struct TcArgs {
   const float *pk_scale, *pk_shift; int pk_relu;  // per OUTPUT channel (nullptr: identity): the consumer's BatchNorm+ReLU
   int pk_fill;                           // zero the rest of a half-written last 32-channel chunk
   int *oflow;                            // device flag: a packed value beyond the fp16 range
-  int nstages, nbstages, tmem_cols, tmem_acols;  // A ring depth (TMEM), weight ring depth (smem), TMEM columns, first A column
-  int ksplit;      // CTAs per cluster along z sharing one tile's iterations (1 = no split)
 };
 
-// Warp roles: warps 0-3 = producer group 0, warps 4-7 = producer group 1 (one output row per thread; group g fills slot g
-// of every iteration pair), warp 8 = MMA issuer (warp-uniform, one elected lane), warp 9 = weight loader (TMA bulk copies).
-// Barriers per pair stage: full (8 producer-warp arrivals), bfull (weights: expect_tx), free (tcgen05.commit);
-// bars[8]: accumulator complete.
-__global__ void __launch_bounds__(TC_THREADS, 2) spconv_tc_kernel(TcArgs p) {
-  extern __shared__ __align__(1024) unsigned char smem[];
-  __shared__ __align__(8) unsigned long long bars[12];  // [0..2] A full, [3..5] pair free, [8] done, [9..11] weights full
-  __shared__ uint32_t s_tmem;
+template <int NT>
+constexpr size_t tc_stage_bytes() { return (size_t)TC_A_BYTES + (size_t)NT * 128; }  // rows + [4 chunks][hi|lo][NT][16 B]
+template <int NT>
+constexpr int tc_min_blocks() { return NT <= 64 ? 2 : 1; }  // register file: 2 x NT / 2 fp32 accumulators per thread
+
+template <int NT>
+__global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<NT>()) spconv_tc_kernel(TcArgs p) {
+  constexpr int R = NT / 2;  // accumulator registers per thread and product
+  extern __shared__ __align__(1024) unsigned char smem_raw[];
   __shared__ unsigned int s_mask;
   __shared__ int s_list[32];
   __shared__ int s_nact;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int warp_u = __shfl_sync(0xffffffffu, warp, 0);  // provably warp-uniform copy for the role dispatch
-  const bool producer = warp < 8;
-  const int grp = warp >> 2;          // producer group (0/1)
-  const int r = tid & (TC_ROWS - 1);  // row of this producer thread
-  const int row0 = blockIdx.x * TC_ROWS;
-  const int my_row = row0 + r;
-  const bool row_ok = producer && my_row < p.Mout;
-  const int N = p.N, NT = p.NT;
-  const int n0 = blockIdx.y * NT;
-  const int nt = min(NT, N - n0);                     // columns of this CTA (multiple of 16)
-  const uint32_t b_bytes = (uint32_t)NT * TC_KC * 2;  // NT * 64 B (fp16)
-  const uint32_t bstage_bytes = 2 * b_bytes;    // weight ring stage: hi + lo
-  const int NS = p.nstages;   // A stages in TMEM (32 columns each) == weight stages in shared memory; even
-  unsigned char *bring = smem;
-  int32_t *map_s = reinterpret_cast<int32_t *>(bring + (size_t)NS * bstage_bytes);  // [K][128] (only when p.map)
+  const int tid = threadIdx.x, lane = tid & 31, wg = tid >> 7, wq = (tid >> 5) & 3;
+  unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // SWIZZLE_128B: 1024-aligned
+  unsigned char *a_ring = smem;
+  unsigned char *b_ring = a_ring + (size_t)TC_STAGES * TC_A_BYTES;
+  int32_t *map_s = reinterpret_cast<int32_t *>(b_ring + (size_t)TC_STAGES * NT * 128);  // [K][128]
+  const uint32_t a_base = smem_u32(a_ring), b_base = smem_u32(b_ring);
+  const int nkc = (p.Cin + TC_KC - 1) / TC_KC;
+  const int ks_last = (p.Cin - (nkc - 1) * TC_KC + 15) >> 4;  // 16-channel k-steps of the last slice (1 or 2)
+  const int S = p.ksplit, z = blockIdx.z;
+  const bool split = S > 1;
 
-  if (tid == 0) {
-    for (int i = 0; i < NS / 2; i++) {
-      mbar_init(smem_u32(&bars[BAR_FULL + i]), 8);  // one arrival per producer warp
-      mbar_init(smem_u32(&bars[BAR_FREE + i]), 1);
-      mbar_init(smem_u32(&bars[BAR_BFULL + i]), 1);
-    }
-    mbar_init(smem_u32(&bars[8]), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    s_mask = 0u;
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&s_tmem)),
-                 "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem = s_tmem;
-
-  // ---- rulebook slice of this tile -> shared memory; which kernel offsets have any active pair ------------
-  if (p.map) {
-    unsigned int flags = 0u;
-    if (producer) {
-      // all of this thread's rulebook entries are requested before the first one is used (one memory latency, not K/2)
-      for (int ob = grp; ob < p.K; ob += 28) {
-        int srcv[14];
+  for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
+    const int tile = item / p.nparts, part = item - tile * p.nparts;
+    const int row0 = tile * TC_ROWS, n0 = part * NT;
+    const int nt = min(NT, p.N - n0);  // columns of this item (multiple of 16)
+    __syncthreads();  // the previous item is done with the rulebook slice and the ring
+    if (tid == 0) s_mask = 0u;
+    __syncthreads();
+    // ---- rulebook slice of this tile -> shared memory; which kernel offsets have any active pair ----------------
+    {
+      const int r = tid & (TC_ROWS - 1), row = row0 + r;
+      unsigned int flags = 0u;
+      if (p.map) {
+        for (int ob = tid >> 7; ob < p.K; ob += 16) {  // up to 8 entries of this row in flight
+          int v[8];
 #pragma unroll
-        for (int j = 0; j < 14; j++) {
-          const int o = ob + 2 * j;
-          srcv[j] = (o < p.K && row_ok) ? __ldg(&p.map[(size_t)o * p.Mout + my_row]) : -1;
-        }
+          for (int j = 0; j < 8; j++) {
+            const int o = ob + 2 * j;
+            v[j] = (o < p.K && row < p.Mout) ? __ldg(&p.map[(size_t)o * p.Mout + row]) : -1;
+          }
 #pragma unroll
-        for (int j = 0; j < 14; j++) {
-          const int o = ob + 2 * j;
-          if (o < p.K) {
-            map_s[o * TC_ROWS + r] = srcv[j];
-            if (srcv[j] >= 0) flags |= 1u << o;
+          for (int j = 0; j < 8; j++) {
+            const int o = ob + 2 * j;
+            if (o < p.K) {
+              map_s[o * TC_ROWS + r] = v[j];
+              if (v[j] >= 0) flags |= 1u << o;
+            }
           }
         }
+      } else if (tid < TC_ROWS) {
+        map_s[r] = row < p.Mout ? row : -1;
+        flags = 1u;
       }
+      flags = __reduce_or_sync(0xffffffffu, flags);
+      if (lane == 0 && flags) atomicOr(&s_mask, flags);
     }
-    flags = __reduce_or_sync(0xffffffffu, flags);
-    if (lane == 0 && flags) atomicOr(&s_mask, flags);
-  }
-  __syncthreads();
-  if (tid < 32) {  // compact the active offsets in ascending order
-    if (p.map) {
+    __syncthreads();
+    if (tid < 32) {  // compact the active offsets in ascending order
       const unsigned int m = s_mask;
       if (tid < p.K && (m >> tid & 1u)) s_list[__popc(m & ((1u << tid) - 1u))] = tid;
       if (tid == 0) s_nact = __popc(m);
-    } else if (tid == 0) {
-      s_list[0] = 0;
-      s_nact = 1;
     }
-  }
-  __syncthreads();
-  const int nkc = (p.Cin + TC_KC - 1) / TC_KC;
-  // split-K: the cluster's CTAs take contiguous shares of the tile's (offset, slice) iterations
-  const int S = p.ksplit, z = blockIdx.z;
-  const int total_all = s_nact * nkc;
-  const int i_beg = (int)((long long)total_all * z / S), i_end = (int)((long long)total_all * (z + 1) / S);
-  const int total = i_end - i_beg;
-  const int a0 = i_beg / nkc, k0 = i_beg - a0 * nkc;  // first iteration of this CTA
+    __syncthreads();
+    // split-K: the cluster's CTAs take contiguous shares of the item's (offset, slice) iterations
+    const int total_all = s_nact * nkc;
+    const int i_beg = (int)((long long)total_all * z / S), i_end = (int)((long long)total_all * (z + 1) / S);
+    const int total = i_end - i_beg;
 
-  // Pipeline unit = a PAIR of consecutive iterations (2P, 2P+1): producer group g fills A stage (ps, g), the loader
-  // brings both weight slices under one transaction barrier, and the MMA thread pays its fixed costs (two barrier
-  // waits, one commit) once per pair and issues up to 8 back-to-back MMAs, which is what lets them pipeline in the
-  // tensor core. Per pair stage ps: full[ps] (8 producer-warp arrivals), bfull[ps] (weights landed),
-  // free[ps] (tcgen05.commit: both the A stages and the weight stages of the pair can be overwritten).
-  const int npairs = (total + 1) >> 1;
-  const int NP = NS >> 1;
-  if (producer) {
-    // ---- packed input: the gather is pure data movement, so the registers hold TWO future iterations of this thread's
-    //      row (4 iterations ahead of the MMA warp counting both groups) -- the L2 latency of the gather is covered
-    //      without shared memory.
-    uint32_t va[32], vb[32];
-    int ia = a0, ikc = k0 + grp;  // issue cursor: (offset list position, channel slice) of the next own iteration to load
-    while (ikc >= nkc) { ikc -= nkc; ia++; }
-    int nload = grp;        // CTA-local iteration index of the next load
-    // One gathered row slice = one 128-byte line, every lane a different line: the loads are tag-bound in L1, so the
-    // slice is fetched with four 256-bit loads (LDG.E.256) instead of eight 128-bit ones.
-    auto load = [&](uint32_t (&buf)[32]) {
-      if (nload < total) {
-        const int o = s_list[ia];
-        const int src = p.map ? map_s[o * TC_ROWS + r] : (row_ok ? my_row : -1);
-        if (src >= 0) {
-          const float *rp = p.in + (size_t)src * p.in_stride + p.in_off + ikc * TC_KC;
+    // ---- gather of iteration `it` (CTA-local) into ring stage it % TC_STAGES: 1024 row chunks + 8 NT weight chunks
+    auto load = [&](int it) {
+      if (it < total) {
+        const int gi = i_beg + it, a = gi / nkc, kc = gi - a * nkc;
+        const int o = s_list[a];
+        const int s = it % TC_STAGES;
+        const uint32_t sa = a_base + (uint32_t)s * TC_A_BYTES;
+        const int32_t *ms = map_s + o * TC_ROWS;
 #pragma unroll
-          for (int q = 0; q < 4; q++)
-            asm volatile("ld.global.nc.v8.u32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                         : "=r"(buf[8 * q + 0]), "=r"(buf[8 * q + 1]), "=r"(buf[8 * q + 2]), "=r"(buf[8 * q + 3]),
-                           "=r"(buf[8 * q + 4]), "=r"(buf[8 * q + 5]), "=r"(buf[8 * q + 6]), "=r"(buf[8 * q + 7])
-                         : "l"(rp + 8 * q));
-        } else {
-#pragma unroll
-          for (int q = 0; q < 32; q++) buf[q] = 0u;
+        for (int q = 0; q < TC_ROWS * 8 / TC_THREADS; q++) {
+          const int c = tid + q * TC_THREADS, row = c >> 3, ch = c & 7;
+          const int src = ms[row];
+          const uint32_t *gp = p.in + (size_t)max(src, 0) * p.in_stride + kc * TC_KC + ch * 4;
+          cp_async16(sa + (uint32_t)(row * 128 + ((ch ^ (row & 7)) << 4)), gp, src >= 0 ? 16 : 0);
+        }
+        const uint32_t sb = b_base + (uint32_t)s * (NT * 128);
+        const float4 *g = reinterpret_cast<const float4 *>(p.Wp) + ((size_t)o * nkc + kc) * (size_t)p.N * 8;
+        for (int c = tid; c < 8 * NT; c += TC_THREADS) {
+          const int seg = c / NT, n = c - seg * NT;  // seg = chunk * 2 + (hi, lo)
+          const bool ok = n < nt;
+          cp_async16(sb + (uint32_t)c * 16u, g + (size_t)seg * p.N + n0 + (ok ? n : 0), ok ? 16 : 0);
         }
       }
-      nload += 2;
-      ikc += 2;
-      while (ikc >= nkc) { ikc -= nkc; ia++; }
+      cp_async_commit();  // (an empty group past the end keeps the group count in step)
     };
-    int ps = 0, u = 0, P = 0;
-    auto consume = [&](uint32_t (&buf)[32]) {
-      const bool work = 2 * P + grp < total;  // an odd tail leaves group 1 without a slice: it only arrives
-      if (u >= 1) mbar_wait(smem_u32(&bars[BAR_FREE + ps]), (uint32_t)((u - 1) & 1));
-      if (work) {
-        const uint32_t ta = tmem + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)(p.tmem_acols + (2 * ps + grp) * 32);
-        tmem_st32(ta, buf);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      // one arrival per WARP (every lane has completed and fenced its own store): 256 per-thread arrivals on one
-      // mbarrier serialise in the shared-memory atomic unit and were the floor of the whole pipeline
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&bars[BAR_FULL + ps]));
-      // Refill this buffer (own iteration +2) only AFTER the arrive: tcgen05.wait::st / tcgen05.fence compile to
-      // FENCE.VIEW.ASYNC, which also waits for every outstanding global load of the thread -- issued before the
-      // fence, the gather's L2 latency was paid in full on every iteration instead of overlapping the other buffer.
-      if (work) load(buf);
-      P++;
-      if (++ps == NP) { ps = 0; u++; }
-    };
-    load(va);
-    load(vb);
-    for (int j = 0; j < npairs; j += 2) {
-      consume(va);
-      if (j + 1 < npairs) consume(vb);
-    }
-  } else if (warp == 9) {
-    // ---- weight loader: one elected lane streams the packed slices with TMA bulk copies (cp.async.bulk, async proxy:
-    //      no generic->async fence needed); completion is signalled on the pair's mbarrier by complete_tx. Global
-    //      layout [chunk q][hi|lo][N][16 B] == shared layout [q][hi nt | lo nt][16 B] when the CTA owns all N columns,
-    //      so a whole slice is ONE bulk copy; with a column split it is one copy per (q, part), one lane each.
-    int ps = 0, ub = 0, kc = k0, a_idx = a0;
-    for (int P = 0; P < npairs; P++) {
-      if (ub >= 1) mbar_wait(smem_u32(&bars[BAR_FREE + ps]), (uint32_t)((ub - 1) & 1));
-      const int nit = min(2, total - 2 * P);
-      const uint32_t bar = smem_u32(&bars[BAR_BFULL + ps]);
-      // slot 0 / slot 1 of the pair: offset, slice, 16-channel k-steps
-      const int o0 = s_list[a_idx], kc0 = kc;
-      int kc1 = kc + 1, a1 = a_idx;
-      if (kc1 == nkc) { kc1 = 0; a1++; }
-      const int o1 = (nit > 1) ? s_list[a1] : 0;
-      const int ks0 = (min(TC_KC, p.Cin - kc0 * TC_KC) + 15) >> 4;
-      const int ks1 = (nit > 1) ? (min(TC_KC, p.Cin - kc1 * TC_KC) + 15) >> 4 : 0;
-      const int nseg0 = 4 * ks0, nseg1 = 4 * ks1;  // (chunk, part) segments of nt*16 bytes
-      if (lane == 0) {
-        const uint32_t bytes = (uint32_t)(nseg0 + nseg1) * (uint32_t)nt * 16u;
-        asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
-      }
-      __syncwarp();
-      const float4 *g0 = reinterpret_cast<const float4 *>(p.Wp) + ((size_t)o0 * nkc + kc0) * (size_t)N * 8;
-      const float4 *g1 = reinterpret_cast<const float4 *>(p.Wp) + ((size_t)o1 * nkc + kc1) * (size_t)N * 8;
-      const uint32_t bb0 = smem_u32(bring + (size_t)(2 * ps) * bstage_bytes), bb1 = bb0 + bstage_bytes;
-      if (nt == N) {
-        if (lane == 0)
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       ::"r"(bb0), "l"(g0), "r"((uint32_t)nseg0 * (uint32_t)nt * 16u), "r"(bar) : "memory");
-        if (lane == 1 && nit > 1)
-          asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                       ::"r"(bb1), "l"(g1), "r"((uint32_t)nseg1 * (uint32_t)nt * 16u), "r"(bar) : "memory");
-      } else if (lane < nseg0 + nseg1) {  // column split: one bulk copy per (chunk, part) segment
-        const bool second = lane >= nseg0;
-        const int sg = second ? lane - nseg0 : lane;
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     ::"r"((second ? bb1 : bb0) + (uint32_t)(sg * nt) * 16u), "l"((second ? g1 : g0) + (size_t)sg * N + n0),
-                     "r"((uint32_t)nt * 16u), "r"(bar)
-                     : "memory");
-      }
-      if (++ps == NP) { ps = 0; ub++; }
-      kc += 2;
-      while (kc >= nkc) { kc -= nkc; a_idx++; }
-    }
-  } else if (warp_u == 8) {
-    // ---- MMA issuer: per 16-channel k-step two instructions
-    //        D[:, 0:2nt]  += A_hi * [B_hi | B_lo]     (N = 2nt)
-    //        D[:, nt:2nt] += A_lo *  B_hi             (N = nt)
-    //      so columns [0,nt) hold hi*hi and [nt,2nt) the two correction products (summed in the epilogue).
-    //      The WHOLE warp runs this loop and one elected lane issues: with warp-uniform control flow and operands the
-    //      compiler keeps descriptors in uniform registers and emits bare UTCHMMA; issued from a divergent
-    //      `lane == 0` branch every instruction was wrapped in an R2UR + VOTEU/ELECT/BRA.U.ANY waterfall loop, and that
-    //      single thread's instruction stream (not the tensor pipe) paced the whole kernel.
-    //      Measured floor (scripts/umma_rate.py, round 2): 151 cycles per k-step (both instructions) for nt = 32..96,
-    //      200 at nt = 128, independent of N below that -- 302 cycles per 32-channel iteration and SM is the tensor
-    //      pipe's issue floor for this operand shape (M = 128, K = 16, A from TMEM).
-    // instruction descriptor: D = f32 (1 << 4), A = B = f16 (format 0), both K-major, N >> 3, M >> 4
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem, 0);
-    const int total_u = __shfl_sync(0xffffffffu, total, 0);
-    const int npairs_u = (total_u + 1) >> 1;
-    const int k0_u = __shfl_sync(0xffffffffu, k0, 0);
-    uint32_t leader;
-    asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(leader));
-    const uint32_t idesc2 = (1u << 4) | ((uint32_t)((2 * nt) >> 3) << 17) | ((uint32_t)(TC_ROWS >> 4) << 24);
-    const uint32_t idesc1 = (1u << 4) | ((uint32_t)(nt >> 3) << 17) | ((uint32_t)(TC_ROWS >> 4) << 24);
-    const uint32_t b_lbo = (uint32_t)(2 * nt) * 16;
-    const uint64_t b_step = (uint64_t)((2 * b_lbo) >> 4);
-    const uint32_t bring_u = smem_u32(bring);
-    const uint32_t bars_u = smem_u32(&bars[0]);
-    const uint32_t acol0 = tmem_u + (uint32_t)p.tmem_acols;
-    uint32_t first = 0u;  // 0 for the very first MMA (overwrite), then 1
-    int ps = 0, kc = k0_u;
-    uint32_t par = 0u;
-    for (int P = 0; P < npairs_u; P++) {
-      mbar_wait(bars_u + 8u * (uint32_t)(BAR_BFULL + ps), par);
-      mbar_wait(bars_u + 8u * (uint32_t)(BAR_FULL + ps), par);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const int nit = min(2, total_u - 2 * P);
-      for (int h = 0; h < nit; h++) {
-        const int kvalid = min(TC_KC, p.Cin - kc * TC_KC);
-        const int ksteps = (kvalid + 15) >> 4;
-        const uint32_t sbt = bring_u + (uint32_t)(2 * ps + h) * bstage_bytes;
-        uint64_t dbb = umma_desc(sbt, b_lbo, 128);
-        uint32_t ah = acol0 + (uint32_t)((2 * ps + h) * 32), al = ah + 16u;
-        for (int ks = 0; ks < ksteps; ks++) {
-          if (leader) {
-            umma_f16_ts(tmem_u, ah, dbb, idesc2, first);
-            umma_f16_ts(tmem_u + (uint32_t)nt, al, dbb, idesc1, 1u);
-          }
-          first = 1u;
-          ah += 8u; al += 8u; dbb += b_step;
-        }
-        if (++kc == nkc) kc = 0;
-      }
-      if (leader) umma_commit(bars_u + 8u * (uint32_t)(BAR_FREE + ps));  // frees both A stages and both weight stages of the pair
-      __syncwarp();
-      if (++ps == NP) { ps = 0; par ^= 1u; }
-    }
-    if (leader && total_u > 0) umma_commit(bars_u + 8u * 8u);
-    __syncwarp();
-  }
-  // ---- epilogue: TMEM lane = output row; warp w reads lanes 32*(w%4).., column half w/4 -----------------
-  const bool split = S > 1;
-  const uint32_t pbuf = smem_u32(bring);  // split-K partial tile [nt columns][128 rows] f32 (the weight ring is idle by now)
-  if (split) {
-    if (producer && z > 0) {
-      if (total > 0) {
-        mbar_wait(smem_u32(&bars[8]), 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      }
-      const int lane_grp = warp & 3, chalf = warp >> 2;
-      const int cbeg = chalf * (nt >> 1), cend = cbeg + (nt >> 1);
-      for (int cb = cbeg; cb < cend; cb += 8) {
-        uint32_t v[8], c[8];
-        if (total > 0) {
-          uint32_t taddr = tmem + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)cb;
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                       : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                       : "r"(taddr));
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                       : "=r"(c[0]), "=r"(c[1]), "=r"(c[2]), "=r"(c[3]), "=r"(c[4]), "=r"(c[5]), "=r"(c[6]), "=r"(c[7])
-                       : "r"(taddr + (uint32_t)nt));
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        } else {
+
+    float acc[R], cor[R];
 #pragma unroll
-          for (int e = 0; e < 8; e++) v[e] = c[e] = 0u;
-        }
+    for (int i = 0; i < R; i++) acc[i] = cor[i] = 0.f;
 #pragma unroll
-        for (int e = 0; e < 8; e++) {
-          const float x = fmaf(__uint_as_float(c[e]), kLoInv, __uint_as_float(v[e]));
-          asm volatile("st.shared.f32 [%0], %1;" ::"r"(pbuf + (uint32_t)(((cb + e) * TC_ROWS + lane_grp * 32 + lane) * 4)), "f"(x) : "memory");
+    for (int s = 0; s < TC_STAGES - 1; s++) load(s);
+    const uint32_t b_lbo = (uint32_t)NT * 32u;  // distance between the two 8-channel chunks of a k-step: [hi NT | lo NT] x 16 B
+    for (int it = 0; it < total; it++) {
+      cp_async_wait<TC_STAGES - 2>();
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy (cp.async) writes -> visible to wgmma
+      __syncthreads();  // every thread's copies of stage it landed; every warpgroup is done with stage it - 1
+      load(it + TC_STAGES - 1);
+      const int s = it % TC_STAGES;
+      const int kc = (i_beg + it) % nkc;
+      const int ksteps = (kc + 1 < nkc) ? 2 : ks_last;
+      const uint32_t sa = a_base + (uint32_t)s * TC_A_BYTES + (uint32_t)wg * (64 * 128);
+      const uint32_t sb = b_base + (uint32_t)s * (NT * 128);
+      wgmma_fence_regs(acc);
+      wgmma_fence_regs(cor);
+      wgmma_fence();
+      for (int ks = 0; ks < ksteps; ks++) {
+        const uint64_t ah = desc_sw128(sa + 32u * ks), al = desc_sw128(sa + 64u + 32u * ks);
+        const uint32_t bk = sb + (uint32_t)ks * 2u * b_lbo;  // chunks 2 ks, 2 ks + 1
+        const uint64_t bh = desc_plain(bk, b_lbo, 128), bl = desc_plain(bk + (uint32_t)NT * 16u, b_lbo, 128);
+        wgmma_f16<NT>(acc, ah, bh);
+        wgmma_f16<NT>(cor, ah, bl);
+        wgmma_f16<NT>(cor, al, bh);
+      }
+      wgmma_commit();
+      wgmma_wait0();
+      wgmma_fence_regs(acc);
+      wgmma_fence_regs(cor);
+    }
+    cp_async_wait<0>();
+#pragma unroll
+    for (int i = 0; i < R; i++) acc[i] = fmaf(cor[i], kLoInv, acc[i]);
+
+    // ---- epilogue: thread holds rows rb, rb + 8 and columns 8 j + 2 (lane & 3) + {0, 1} of its warpgroup's 64 rows --
+    const int rl = wg * 64 + wq * 16 + (lane >> 2);  // tile-local row of acc[4 j + 0, 1]; acc[4 j + 2, 3] is rl + 8
+    const int cl = 2 * (lane & 3);
+    if (split) {
+      const uint32_t pbuf = a_base;  // partial tile [NT columns][128 rows] f32 (the ring is idle by now)
+      __syncthreads();
+      if (z > 0) {
+#pragma unroll
+        for (int i = 0; i < R; i++) {
+          const int col = 8 * (i >> 2) + cl + (i & 1), row = rl + 8 * ((i >> 1) & 1);
+          asm volatile("st.shared.f32 [%0], %1;" ::"r"(pbuf + (uint32_t)((col * TC_ROWS + row) * 4)), "f"(acc[i]) : "memory");
         }
       }
-    }
-    __syncwarp();
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  }
-  if (producer && (!split || z == 0)) {
-    if (total > 0) {
-      mbar_wait(smem_u32(&bars[8]), 0);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    }
-    const int lane_grp = warp & 3, chalf = warp >> 2;
-    const int row = row0 + lane_grp * 32 + lane;
-    const int cbeg = chalf * (nt >> 1), cend = cbeg + (nt >> 1);
-    for (int cb = cbeg; cb < cend; cb += 8) {
-      uint32_t v[8], c[8];
-      if (total > 0) {
-        uint32_t taddr = tmem + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)cb;
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                     : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                     : "r"(taddr));
-        asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-                     : "=r"(c[0]), "=r"(c[1]), "=r"(c[2]), "=r"(c[3]), "=r"(c[4]), "=r"(c[5]), "=r"(c[6]), "=r"(c[7])
-                     : "r"(taddr + (uint32_t)nt));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int e = 0; e < 8; e++) v[e] = __float_as_uint(fmaf(__uint_as_float(c[e]), kLoInv, __uint_as_float(v[e])));
-      } else {
-#pragma unroll
-        for (int e = 0; e < 8; e++) v[e] = 0u;
-      }
-      if (split) {  // add the other ranks' partial tiles in rank order (distributed shared memory)
+      asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+      if (z == 0) {  // add the other ranks' partial tiles in rank order (distributed shared memory)
         for (int zz = 1; zz < S; zz++) {
           uint32_t rbase;
           asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rbase) : "r"(pbuf), "r"(zz));
-          float t[8];
 #pragma unroll
-          for (int e = 0; e < 8; e++)
-            asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(t[e]) : "r"(rbase + (uint32_t)(((cb + e) * TC_ROWS + lane_grp * 32 + lane) * 4)) : "memory");
-#pragma unroll
-          for (int e = 0; e < 8; e++) v[e] = __float_as_uint(__uint_as_float(v[e]) + t[e]);
+          for (int i = 0; i < R; i++) {
+            const int col = 8 * (i >> 2) + cl + (i & 1), row = rl + 8 * ((i >> 1) & 1);
+            float t;
+            asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(t) : "r"(rbase + (uint32_t)((col * TC_ROWS + row) * 4)) : "memory");
+            acc[i] += t;
+          }
         }
       }
-      if (row < p.Mout) {
-        const int col = n0 + cb;
-        const float *rp = p.residual ? p.residual + (size_t)row * p.res_stride + p.res_off + col : nullptr;
-        float x[8];
+      // ranks > 0 keep their shared memory alive until rank 0 has read it
+      asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+    }
+    if (!split || z == 0) {
 #pragma unroll
-        for (int e = 0; e < 8; e++) x[e] = __uint_as_float(v[e]);
-        const bool full = col + 8 <= p.Cout;
-        if (p.bias) {
+      for (int h = 0; h < 2; h++) {
+        const int row = row0 + rl + 8 * h;
+        if (row >= p.Mout) continue;
 #pragma unroll
-          for (int e = 0; e < 8; e++)
-            if (col + e < p.Cout) x[e] += __ldg(&p.bias[col + e]);
-        }
-        if (rp) {
-          if (full && ((reinterpret_cast<uintptr_t>(rp) & 15) == 0)) {
-            const float4 r0 = __ldg(reinterpret_cast<const float4 *>(rp)), r1 = __ldg(reinterpret_cast<const float4 *>(rp) + 1);
-            x[0] += r0.x; x[1] += r0.y; x[2] += r0.z; x[3] += r0.w;
-            x[4] += r1.x; x[5] += r1.y; x[6] += r1.z; x[7] += r1.w;
-          } else {
+        for (int j = 0; j < NT / 8; j++) {
+          const int cj = 8 * j + cl;  // item-local column of this pair
+          if (cj >= nt) continue;
+          const int col = n0 + cj;
+          float x[2] = {acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]};
+          const bool full = col + 2 <= p.Cout;
+          if (p.bias) {
 #pragma unroll
-            for (int e = 0; e < 8; e++)
+            for (int e = 0; e < 2; e++)
+              if (col + e < p.Cout) x[e] += __ldg(&p.bias[col + e]);
+          }
+          if (p.residual) {
+            const float *rp = p.residual + (size_t)row * p.res_stride + p.res_off + col;
+#pragma unroll
+            for (int e = 0; e < 2; e++)
               if (col + e < p.Cout) x[e] += __ldg(rp + e);
           }
+          if (p.out) {
+            float *op = p.out + (size_t)row * p.out_stride + p.out_off + col;
+            if (full && ((reinterpret_cast<uintptr_t>(op) & 7) == 0)) {
+              *reinterpret_cast<float2 *>(op) = make_float2(x[0], x[1]);
+            } else {
+#pragma unroll
+              for (int e = 0; e < 2; e++)
+                if (col + e < p.Cout) op[e] = x[e];
+            }
+          }
+          if (p.pk) {
+            // the consumer's BatchNorm(eval)+ReLU, then the fp16 hi/lo split: 2 channels -> 1 word hi + 1 word lo
+            float y[2];
+            bool big = false;
+#pragma unroll
+            for (int e = 0; e < 2; e++) {
+              float t = x[e];
+              if (col + e >= p.Cout) t = 0.f;  // padding channels stay exactly zero
+              else if (p.pk_scale) t = fmaf(t, __ldg(&p.pk_scale[col + e]), __ldg(&p.pk_shift[col + e]));
+              if (p.pk_relu) t = fmaxf(t, 0.f);
+              big |= !(fabsf(t) <= 65504.f);
+              y[e] = t;
+            }
+            if (big) *p.oflow = 1;
+            const __half2 hh = f2h2_sat(y[0], y[1]);
+            const float2 hf = __half22float2(hh);
+            const __half2 ll = f2h2_sat((y[0] - hf.x) * kLoScale, (y[1] - hf.y) * kLoScale);
+            const int ch = p.pk_coff + col;  // channel in the packed tensor (even)
+            uint32_t *dst = p.pk + (size_t)row * p.pk_stride + (ch >> 5) * 32 + ((ch & 31) >> 1);
+            dst[0] = *reinterpret_cast<const uint32_t *>(&hh);
+            dst[16] = *reinterpret_cast<const uint32_t *>(&ll);
+          }
         }
-        if (p.out) {
-          float *op = p.out + (size_t)row * p.out_stride + p.out_off + col;
-          if (full && ((reinterpret_cast<uintptr_t>(op) & 15) == 0)) {
-            reinterpret_cast<float4 *>(op)[0] = make_float4(x[0], x[1], x[2], x[3]);
-            reinterpret_cast<float4 *>(op)[1] = make_float4(x[4], x[5], x[6], x[7]);
-          } else {
-#pragma unroll
-            for (int e = 0; e < 8; e++)
-              if (col + e < p.Cout) op[e] = x[e];
-          }
-        }
-        if (p.pk) {
-          // the consumer's BatchNorm(eval)+ReLU, then the fp16 hi/lo split: 8 channels -> 4 words hi + 4 words lo
-          float y[8];
-          bool big = false;
-#pragma unroll
-          for (int e = 0; e < 8; e++) {
-            float t = x[e];
-            if (col + e >= p.Cout) t = 0.f;  // padding channels stay exactly zero
-            else if (p.pk_scale) t = fmaf(t, __ldg(&p.pk_scale[col + e]), __ldg(&p.pk_shift[col + e]));
-            if (p.pk_relu) t = fmaxf(t, 0.f);
-            big |= !(fabsf(t) <= 65504.f);
-            y[e] = t;
-          }
-          if (big) *p.oflow = 1;
-          uint32_t hw[4], lw[4];
-#pragma unroll
-          for (int q = 0; q < 4; q++) {
-            const __half2 h = f2h2_sat(y[2 * q], y[2 * q + 1]);
-            const float2 hf = __half22float2(h);
-            const __half2 l = f2h2_sat((y[2 * q] - hf.x) * kLoScale, (y[2 * q + 1] - hf.y) * kLoScale);
-            hw[q] = *reinterpret_cast<const uint32_t *>(&h);
-            lw[q] = *reinterpret_cast<const uint32_t *>(&l);
-          }
-          const int ch = p.pk_coff + col;  // channel in the packed tensor (multiple of 8)
-          uint32_t *dst = p.pk + (size_t)row * p.pk_stride + (ch >> 5) * 32 + ((ch & 31) >> 1);
-          *reinterpret_cast<uint4 *>(dst) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
-          *reinterpret_cast<uint4 *>(dst + 16) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
-          if (col + 8 == N && (N & 31) && p.pk_fill) {
-            // N = Cout rounded to 16 ends in the middle of a 32-channel chunk: the consumer reads whole chunks, so the
-            // upper half must be zero (not stale memory: 0 * NaN would poison the sums)
-            const int ch2 = p.pk_coff + N;
-            uint32_t *zp = p.pk + (size_t)row * p.pk_stride + (ch2 >> 5) * 32 + ((ch2 & 31) >> 1);
-            const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
-            reinterpret_cast<uint4 *>(zp)[0] = zero; reinterpret_cast<uint4 *>(zp)[1] = zero;
-            reinterpret_cast<uint4 *>(zp + 16)[0] = zero; reinterpret_cast<uint4 *>(zp + 16)[1] = zero;
-          }
+        if (p.pk && p.pk_fill && n0 + nt == p.N && (p.N & 31)) {
+          // N = Cout rounded to 16 ends in the middle of a 32-channel chunk: the consumer reads whole chunks, so the
+          // upper 16 channels (8 words hi + 8 words lo) must be zero (not stale memory: 0 * NaN would poison the sums);
+          // the 4 threads of the row write 2 + 2 words each
+          const int ch2 = p.pk_coff + p.N;
+          uint32_t *zp = p.pk + (size_t)row * p.pk_stride + (ch2 >> 5) * 32 + ((ch2 & 31) >> 1) + cl;
+          zp[0] = 0u; zp[1] = 0u; zp[16] = 0u; zp[17] = 0u;
         }
       }
     }
-  }
-  if (split) {  // ranks > 0 keep their shared memory alive until rank 0 has read it
-    __syncwarp();
-    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"((uint32_t)p.tmem_cols) : "memory");
   }
 }
 
@@ -525,7 +330,7 @@ namespace {
 
 int *g_oflow[16] = {nullptr};  // per device: flag raised by the packing code when a value leaves the fp16 range
 
-struct DevInfo { int sms; bool attr_set; bool ss_attr_set; };
+struct DevInfo { int sms; bool attr_set[9]; int per_sm[9]; };  // per NT / 16: shared-memory attribute set, CTAs per SM
 DevInfo g_dev[16] = {};
 
 int current_device(int *dev) {
@@ -547,15 +352,68 @@ int ensure_device(int dev) {
   return SGB_OK;
 }
 
-// Which kernel runs a problem (launch-by-launch A/B inside the real 150k-point step, profiles/r2_conv_launch_ab.txt): the
-// persistent shared-memory-ring kernel (spconv_ss.cu) wins from 16 row tiles upwards when Cout >= 64 (levels 1-4 of the
-// U-Net: -5 % ... -40 %) and on the big 32-channel levels; the register-gather kernel keeps the deep levels (a handful of
-// row tiles: column split + split-K clusters) and the 32-channel tiny U-Net (a few hundred tiles, +10 % there).
-bool use_ss_kernel(int K, int Mout, int Cin, int Cout, int sms) {
-  int plan[5];
-  if (!spconv_ss_plan(K, Mout, Cin, Cout, sms, plan)) return false;
+// Columns per work item of the persistent launch: all of N up to 128, else N cut into equal parts (multiple of 16).
+int persistent_nt(int N) { return N <= 128 ? N : (div_up(N, div_up(N, 128)) + 15) / 16 * 16; }
+
+// Shared memory of a CTA: the gather ring, the rulebook slice of the largest kernel (27 offsets) and the alignment slack.
+size_t tc_smem_bytes(int NT) { return (size_t)TC_STAGES * ((size_t)TC_A_BYTES + (size_t)NT * 128) + 27 * TC_ROWS * 4 + 1024; }
+
+// Which launch runs a problem. The persistent form takes the levels with many row tiles (Cout >= 64 from 16 row tiles
+// upwards, and the big 32-channel levels); one CTA per work item keeps the deep levels (a handful of row tiles: column
+// split + split-K clusters) and the 32-channel tiny U-Net (a few hundred tiles).
+bool use_persistent(int K, int Mout, int Cin, int Cout, int sms) {
+  if ((Cout + 15) / 16 * 16 > 256 || Cin > 512 || K > 27) return false;
   const int tiles = div_up(Mout, TC_ROWS);
   return tiles >= 16 && (Cout >= 64 || tiles >= 4 * sms);
+}
+
+template <int NT>
+int launch_nt(const TcArgs &p, bool persistent, int dev, cudaStream_t stream) {
+  const size_t smem = tc_smem_bytes(NT);
+  DevInfo &d = g_dev[dev];
+  if (!d.attr_set[NT / 16]) {
+    SGB_CUDA_CHECK(cudaFuncSetAttribute(spconv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int n = 0;
+    SGB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, spconv_tc_kernel<NT>, TC_THREADS, smem));
+    d.per_sm[NT / 16] = std::max(n, 1);
+    d.attr_set[NT / 16] = true;
+  }
+  if (persistent) {
+    const int grid = std::min(p.items, d.sms * d.per_sm[NT / 16]);
+    spconv_tc_kernel<NT><<<grid, TC_THREADS, smem, stream>>>(p);
+  } else if (p.ksplit == 1) {
+    spconv_tc_kernel<NT><<<p.items, TC_THREADS, smem, stream>>>(p);
+  } else {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(p.items, 1, p.ksplit);
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 1;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = p.ksplit;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    SGB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, spconv_tc_kernel<NT>, p));
+  }
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+int launch(int NT, const TcArgs &p, bool persistent, int dev, cudaStream_t stream) {
+  switch (NT) {
+    case 16: return launch_nt<16>(p, persistent, dev, stream);
+    case 32: return launch_nt<32>(p, persistent, dev, stream);
+    case 48: return launch_nt<48>(p, persistent, dev, stream);
+    case 64: return launch_nt<64>(p, persistent, dev, stream);
+    case 80: return launch_nt<80>(p, persistent, dev, stream);
+    case 96: return launch_nt<96>(p, persistent, dev, stream);
+    case 112: return launch_nt<112>(p, persistent, dev, stream);
+    case 128: return launch_nt<128>(p, persistent, dev, stream);
+  }
+  SGB_REQUIRE(false, SGB_ERR_RANGE, "spconv_forward_tc: columns per CTA not a multiple of 16 in [16, 128]");
 }
 
 }  // namespace
@@ -605,8 +463,9 @@ long long sgb_spconv_tc_packed_floats(int K, int Cin, int Cout) {
   return (long long)K * nkc * 4 * 2 * N * 4;  // fp16: 4 chunks of 8 halves, counted in 32-bit words
 }
 
-// Tile configuration chosen for a problem (pure function of the sizes; also what the launch uses): for tests and tools.
-// out[0] = NT, [1] = column parts, [2] = split-K ranks, [3] = TMEM columns, [4] = pipeline stages, [5] = row tiles
+// Tile configuration of the one-CTA-per-item launch for a problem (pure function of the sizes; also what the launch
+// uses): for tests and tools. out[0] = NT, [1] = column parts, [2] = split-K ranks, [3] = shared memory per CTA (bytes),
+// [4] = gather ring stages, [5] = row tiles
 int sgb_spconv_tc_plan(int K, int Mout, int Cin, int Cout, int has_map, int sms, int *out) {
   SGB_REQUIRE(out && K >= 1 && Mout >= 1 && Cin >= 1 && Cout >= 1, SGB_ERR_ARG, "spconv_tc_plan arguments");
   if (sms <= 0) sms = kNumSMs;
@@ -614,40 +473,28 @@ int sgb_spconv_tc_plan(int K, int Mout, int Cin, int Cout, int has_map, int sms,
   // Column split: few row tiles (deep U-Net levels) would leave most SMs idle and make one CTA stream all the
   // weights, so N is cut into NT-column CTAs until the grid covers the machine (NT multiple of 16, >= 32).
   const int tiles = div_up(Mout, TC_ROWS);
-  int NT = std::min(N, 128);  // [B_hi | B_lo] is one operand with 2*NT <= 256 columns
+  int NT = std::min(N, 128);
   if (N > 128) NT = (N / 2 + 15) / 16 * 16;
   while (NT > 32 && tiles * div_up(N, NT) < sms) {
     int nxt = (NT / 2 + 15) / 16 * 16;
     if (nxt >= NT) break;
     NT = nxt;
   }
-  const size_t bstage = 2 * (size_t)NT * TC_KC * 2;  // weight ring stage (fp16 hi + lo) in shared memory
-  // TMEM budget: accumulator [main | corrections] = 2*NT columns, then the A ring (32 columns per stage: hi + lo pairs;
-  // an even number of stages because the pipeline moves in pairs). 256 columns (two CTAs per SM) when that leaves
-  // >= 4 stages (two pairs, so gathers overlap the MMAs), else all 512. The weight ring has the same number of stages.
-  const int acols0 = (2 * NT + 31) / 32 * 32;
-  int tmem_cols = 256;
-  int ns = ((256 - acols0) / 32) & ~1;
-  if (ns < 4) { tmem_cols = 512; ns = ((512 - acols0) / 32) & ~1; }
-  ns = std::min(ns, 6);
-  const size_t ring_cap = (tmem_cols == 256) ? 64 * 1024 : 100 * 1024;  // one CTA per SM when it owns all of TMEM
-  while (ns > 2 && (size_t)ns * bstage > ring_cap) ns -= 2;
   // split-K: when even the narrowest column split leaves most SMs idle, a cluster of S CTAs shares each tile's
   // iterations (S <= 8, the portable cluster size) and reduces through distributed shared memory.
   const int nkc = (Cin + TC_KC - 1) / TC_KC;
   const int ctas = tiles * div_up(N, NT);
   int S = 1;
-  if (ctas * 2 <= sms && tmem_cols == 256 && (size_t)ns * bstage >= (size_t)NT * TC_ROWS * 4)
-    S = std::max(1, std::min({8, 2 * sms / ctas, std::max(1, K * nkc / 4)}));
-  out[0] = NT; out[1] = div_up(N, NT); out[2] = S; out[3] = tmem_cols; out[4] = ns; out[5] = tiles;
+  if (ctas * 2 <= sms) S = std::max(1, std::min({8, 2 * sms / ctas, std::max(1, K * nkc / 4)}));
+  out[0] = NT; out[1] = div_up(N, NT); out[2] = S; out[3] = (int)tc_smem_bytes(NT); out[4] = TC_STAGES; out[5] = tiles;
   (void)has_map;
   return SGB_OK;
 }
 
-// 1 = the persistent shared-memory-ring kernel would run this problem, 0 = the register-gather kernel (pure function).
+// 1 = the persistent launch would run this problem, 0 = one CTA per work item (pure function).
 int sgb_spconv_kernel_choice(int K, int Mout, int Cin, int Cout, int sms) {
   if (K < 1 || Mout < 1 || Cin < 1 || Cout < 1) return 0;
-  return use_ss_kernel(K, Mout, Cin, Cout, sms > 0 ? sms : kNumSMs) ? 1 : 0;
+  return use_persistent(K, Mout, Cin, Cout, sms > 0 ? sms : kNumSMs) ? 1 : 0;
 }
 
 int sgb_spconv_forward_tc(const float *d_in_pk, int in_stride, int Min, const int32_t *d_map, int K, int Mout,
@@ -666,7 +513,7 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
                              int pk_coff, const float *d_pk_scale, const float *d_pk_shift, int pk_relu, int pk_fill, int kernel,
                              void *stream) {
   if (Mout == 0 || Cout == 0) return SGB_OK;
-  SGB_REQUIRE(kernel >= -1 && kernel <= 1, SGB_ERR_ARG, "kernel: -1 (choose), 0 (register gather), 1 (shared-memory ring)");
+  SGB_REQUIRE(kernel >= -1 && kernel <= 1, SGB_ERR_ARG, "kernel: -1 (choose), 0 (one CTA per work item), 1 (persistent)");
   SGB_REQUIRE(d_in_pk && d_Wp && (d_out || d_pk_out) && K >= 1 && K <= 27 && Mout > 0 && Min > 0 && Cin > 0 && Cout > 0, SGB_ERR_ARG,
               "spconv_forward_tc arguments");
   SGB_REQUIRE(d_map || (K == 1 && Min >= Mout), SGB_ERR_ARG, "identity map requires K == 1");
@@ -683,15 +530,9 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
   if (rc) return rc;
   rc = ensure_device(dev);
   if (rc) return rc;
-  if (kernel == 1 || (kernel == -1 && use_ss_kernel(K, Mout, Cin, Cout, g_dev[dev].sms)))
-    return spconv_ss_launch(d_in_pk, in_stride, d_map, K, Mout, d_Wp, Cin, Cout, d_residual, res_stride, res_off, d_bias, d_out,
-                            out_stride, out_off, d_pk_out, pk_stride, pk_coff, d_pk_scale, d_pk_shift, pk_relu, pk_fill,
-                            g_oflow[dev], g_dev[dev].sms, &g_dev[dev].ss_attr_set, (cudaStream_t)stream);
-  int plan[6];
-  rc = sgb_spconv_tc_plan(K, Mout, Cin, Cout, d_map != nullptr, g_dev[dev].sms, plan);
-  if (rc) return rc;
+  const bool persistent = kernel == 1 || (kernel == -1 && use_persistent(K, Mout, Cin, Cout, g_dev[dev].sms));
   TcArgs p;
-  p.in = d_in_pk; p.in_stride = in_stride; p.in_off = 0;
+  p.in = (const uint32_t *)d_in_pk; p.in_stride = in_stride;
   p.map = d_map; p.K = K; p.Mout = Mout;
   p.Wp = d_Wp; p.Cin = Cin; p.N = N; p.Cout = Cout;
   p.residual = d_residual; p.res_stride = res_stride; p.res_off = res_off;
@@ -700,41 +541,20 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
   p.pk = (uint32_t *)d_pk_out; p.pk_stride = pk_stride; p.pk_coff = pk_coff;
   p.pk_scale = d_pk_scale; p.pk_shift = d_pk_shift; p.pk_relu = pk_relu; p.pk_fill = pk_fill;
   p.oflow = g_oflow[dev];
-  const int NT = plan[0], S = plan[2], tiles = plan[5];
-  p.NT = NT;
-  p.tmem_cols = plan[3];
-  p.nstages = p.nbstages = plan[4];
-  p.tmem_acols = (2 * NT + 31) / 32 * 32;
-  p.ksplit = S;
-  const size_t bstage = 2 * (size_t)NT * TC_KC * 2;
-  const size_t map_bytes = d_map ? (size_t)K * TC_ROWS * 4 : 0;
-  // at least 77 KB per CTA: never more than two CTAs per SM, so a third CTA cannot sit in tcgen05.alloc behind clusters
-  // whose other ranks wait at barrier.cluster (each CTA holds >= 256 of the 512 TMEM columns until it exits)
-  const size_t smem = std::max(bstage * p.nbstages + map_bytes + 1024, (size_t)77 * 1024);
-  if (!g_dev[dev].attr_set) {
-    SGB_CUDA_CHECK(cudaFuncSetAttribute(spconv_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(160 * 1024)));
-    SGB_CUDA_CHECK(cudaFuncSetAttribute(spconv_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-    g_dev[dev].attr_set = true;
-  }
-  dim3 grid(tiles, plan[1], S);
-  if (S == 1) {
-    spconv_tc_kernel<<<grid, TC_THREADS, smem, (cudaStream_t)stream>>>(p);
+  const int tiles = div_up(Mout, TC_ROWS);
+  int NT;
+  if (persistent) {
+    NT = persistent_nt(N);
+    p.ksplit = 1;
   } else {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = (cudaStream_t)stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = S;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    SGB_CUDA_CHECK(cudaLaunchKernelEx(&cfg, spconv_tc_kernel, p));
+    int plan[6];
+    rc = sgb_spconv_tc_plan(K, Mout, Cin, Cout, d_map != nullptr, g_dev[dev].sms, plan);
+    if (rc) return rc;
+    NT = plan[0];
+    p.ksplit = plan[2];
   }
-  SGB_LAUNCH_CHECK();
-  return SGB_OK;
+  p.nparts = div_up(N, NT);
+  p.items = tiles * p.nparts;
+  return launch(NT, p, persistent, dev, (cudaStream_t)stream);
 }
 }

@@ -1,6 +1,6 @@
 // unet.cu -- executor of a compiled sparse U-Net plan: the ~170 convolution / pack launches of one backbone pass issued
 // from ONE C call instead of ~170 Python->ctypes round trips (the host side of the forward was the bottleneck once the
-// kernels got faster: Python spent ~40 us per convolution, the GPU ~25-60 us).
+// kernels got faster: Python spent longer per convolution than the GPU).
 // The plan is data: softgroup_b200/model/unet_plan.py walks the module tree of the reference-shaped model
 // (softgroup/model/blocks.py:44-143 -- ResidualBlock / UBlock) once and emits one record per launch, with the same fusion
 // decisions as the module path (BatchNorm+ReLU of the consumer folded into the producing conv's epilogue, packed

@@ -68,8 +68,7 @@ class ScanPipeline(object):
     def __init__(self, model, workers=2, freeze_gc=False):
         """freeze_gc: move everything alive now (model, compiled plans, cached tensors) to the permanent generation of Python's
         cyclic GC (gc.collect(); gc.freeze()). The scan threads share the interpreter lock, so a full collection stalls ALL
-        scans in flight for 10-20 ms; with the long-lived objects frozen the collections stay cheap (end to end with 3 in
-        flight: 9.5-10.8 -> 7.6-8.1 ms per 150k-point scan). Off by default: it is a process-wide policy."""
+        scans in flight; with the long-lived objects frozen the collections stay cheap. Off by default: it is a process-wide policy."""
         import concurrent.futures
         import threading
         if freeze_gc:

@@ -3,7 +3,7 @@
 Same names, argument meaning and return layout as softgroup/ops/functions.py of the reference
 (thangvubk/SoftGroup): ball_query, ballquery_batch_p, bfs_cluster, voxelization_idx, voxelization,
 global_avg_pool, sec_mean/min/max, get_mask_iou_on_cluster, get_mask_iou_on_pred, get_mask_label.
-Every op runs in hand-written sm_100a CUDA behind the C ABI of include/sgb200.h; nothing here computes
+Every op runs in hand-written sm_90a CUDA behind the C ABI of include/sgb200.h; nothing here computes
 on the CPU except `voxelization_idx` on CPU tensors (the reference runs it inside DataLoader workers,
 softgroup/data/custom.py:239) which calls the library's C++ host path.
 

@@ -146,8 +146,8 @@ def build_down_map(indices, spatial_shape):
     return out_indices, mp, inv, [int(s) // 2 for s in spatial_shape]
 
 
-CONV_IMPL = os.environ.get('SGB_CONV_IMPL', 'tc')  # 'tc' = tcgen05 tensor cores (default), 'ffma' = CUDA-core fp32 (A/B only)
-# which of the two tcgen05 kernels the module path asks for: -1 = the library chooses (sgb_spconv_kernel_choice), 0 = register
+CONV_IMPL = os.environ.get('SGB_CONV_IMPL', 'tc')  # 'tc' = wgmma tensor cores (default), 'ffma' = CUDA-core fp32 (A/B only)
+# which of the two launches of the tensor-core kernel the module path asks for: -1 = the library chooses (sgb_spconv_kernel_choice), 0 = register
 # gather, 1 = persistent shared-memory ring. Parity tests run every case under 0 and 1; the compiled plan always uses -1.
 CONV_KERNEL = -1
 
@@ -170,7 +170,7 @@ def pack_weight_tc(W):
 
 class WeightPack(object):
     """Weight of one conv in the kernels' formats: .kio [K,Cin,Cout] (CUDA-core kernel) and .tc(), the packed fp16
-    hi/lo split of the tcgen05 kernel."""
+    hi/lo split of the tensor-core kernel."""
     __slots__ = ('kio', 'packed')
 
     def __init__(self, kio):
@@ -205,7 +205,7 @@ def act_pack(feats, in_stride, in_off, C, act=None, relu=None, out=None, out_cof
 
 
 def check_overflow():
-    """The tcgen05 path carries activations as fp16 hi/lo pairs: a packed value beyond the fp16 range (|y| > 65504, or NaN)
+    """The tensor-core path carries activations as fp16 hi/lo pairs: a packed value beyond the fp16 range (|y| > 65504, or NaN)
     cannot be represented. The packing code raises a per-device flag instead of saturating silently; this reads and clears
     it (a blocking 4-byte read on the current stream -- call it where the host waits anyway) and raises."""
     import ctypes
@@ -230,7 +230,7 @@ class Emit(object):
 
 def conv_forward(feats, in_stride, in_off, mp, K, Mout, W, Cin, Cout, act=None, residual=None, bias=None, out=None,
                  out_stride=None, out_off=0, packed_in=None, emit=None, want_fp32=True, m_in=None):
-    """Thin wrapper over sgb_spconv_forward_tc (tcgen05) / sgb_spconv_forward (CUDA cores: SGB_CONV_IMPL=ffma, or shapes
+    """Thin wrapper over sgb_spconv_forward_tc (wgmma) / sgb_spconv_forward (CUDA cores: SGB_CONV_IMPL=ffma, or shapes
     outside the tensor path). W: WeightPack or [K, Cin, Cout] f32 tensor. act: (scale, shift) or None.
     Tensor path: packed_in = the input already activated + packed (feats may then be None, m_in = its row count);
     emit = Emit(...) makes the epilogue write the consumer's packed input; want_fp32 = False skips the fp32 rows

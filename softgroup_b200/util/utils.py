@@ -18,7 +18,7 @@ def cuda_cast(func):
 
 
 def force_fp32(apply_to=None, out_fp16=False):
-    """The B200 path computes in fp32 throughout; kept so decorated methods read like the reference's.
+    """The GPU path computes in fp32 throughout; kept so decorated methods read like the reference's.
     Half inputs (from a caller using autocast) are widened."""
 
     def deco(old_func):

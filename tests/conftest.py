@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on an H100 with -m gpu)')
 
 
 def pytest_collection_modifyitems(config, items):
@@ -40,28 +40,6 @@ def ref_ops():
         return load_ref()
     except Exception:
         return None
-
-
-@pytest.fixture(scope='session')
-def ref_model_module():
-    """The UNMODIFIED reference `softgroup/model/softgroup.py`, imported on top of this repo's spconv / ops shims
-    (build container only; None where /root/reference is absent)."""
-    ref_root = '/root/reference'
-    if not os.path.isdir(ref_root):
-        return None
-    import importlib
-    import types
-    import softgroup_b200
-    softgroup_b200.install_as_reference_backends()
-    pkg = types.ModuleType('softgroup')
-    pkg.__path__ = [os.path.join(ref_root, 'softgroup')]
-    sys.modules.setdefault('softgroup', pkg)
-    util = types.ModuleType('softgroup.util')
-    from softgroup_b200 import util as our_util
-    for n in ('cuda_cast', 'force_fp32', 'rle_decode', 'rle_encode'):
-        setattr(util, n, getattr(our_util, n))
-    sys.modules.setdefault('softgroup.util', util)
-    return importlib.import_module('softgroup.model.softgroup')
 
 
 @pytest.fixture

@@ -1,7 +1,7 @@
 """The CUDA forward against the reference-generated fixture tests/golden/ref_forward_c1.npz (the reference's own
 `forward_test`, softgroup/model/softgroup.py:300-361, run on CPU stand-ins by tests/golden/make_forward_golden.py):
 backbone + heads, then grouping / clusters_voxelization / tiny U-Net / instance heads from the fixture's
-intermediates. First run on a B200 in round 2 (2 passed)."""
+intermediates."""
 import os
 import sys
 

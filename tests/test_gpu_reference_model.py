@@ -1,7 +1,7 @@
 """Drop-in proof on hardware (SURVEY.md 8b, VERDICT round 1 row g1): the UNMODIFIED reference `SoftGroup` class
 (softgroup/model/softgroup.py + blocks.py, staged verbatim into the git-ignored oracle/_ref/pyref by
 oracle/build_ref.py) is instantiated on `softgroup_b200.install_as_reference_backends()` -- this repo's `spconv.pytorch`
-and `softgroup.ops` -- moved to the B200 and called exactly like tools/test.py:145-152 does (`model(batch)` on the
+and `softgroup.ops` -- moved to the GPU and called exactly like tools/test.py:145-152 does (`model(batch)` on the
 dataloader's collated batch). Its result dict is compared with
 
   * this repo's restructured `softgroup_b200.model.SoftGroup` with the same weights on the same scan: proposals / masks

@@ -10,8 +10,8 @@ from softgroup_b200.configs import model_cfg
 from softgroup_b200.model import SoftGroup
 
 pytestmark = pytest.mark.gpu
-# per-conv tolerance (relative to the output scale, vs the float64-accumulating oracle): the tcgen05 path carries every
-# operand as fp16 hi + fp16 lo and evaluates hi*hi + hi*lo + lo*hi with fp32 accumulation in TMEM (~2^-22 per product,
+# per-conv tolerance (relative to the output scale, vs the float64-accumulating oracle): the tensor-core path carries every
+# operand as fp16 hi + fp16 lo and evaluates hi*hi + hi*lo + lo*hi with fp32 accumulation in wgmma (~2^-22 per product,
 # 2^-25 absolute once lo is subnormal); the CUDA-core path is plain fp32 FFMA. Both far inside the 1e-4 end-to-end bar.
 TOL = 5e-5
 
@@ -22,8 +22,9 @@ def _cuda(a):
 
 @pytest.fixture(params=[0, 1], ids=['register_gather', 'smem_ring'])
 def conv_kernel(request):
-    """Every single-convolution parity case runs under both tcgen05 kernels (spconv_tc.cu / spconv_ss.cu), named explicitly
-    through sgb_spconv_forward_tc_ex, whatever sgb_spconv_kernel_choice would pick for the size."""
+    """Every single-convolution parity case runs under both launches of the tensor-core kernel (spconv_tc.cu: one CTA per
+    work item / persistent), named explicitly through sgb_spconv_forward_tc_ex, whatever sgb_spconv_kernel_choice would pick
+    for the size."""
     from softgroup_b200.spconv import core
     old = core.CONV_KERNEL
     core.CONV_KERNEL = request.param
@@ -123,8 +124,9 @@ def _rel_elem(got, want):
 @pytest.mark.parametrize('Cin,Cout,n_rows', [(32, 32, 40000), (64, 64, 24000), (96, 96, 24000), (128, 128, 20000),
                                              (192, 96, 20000), (64, 32, 40000), (224, 224, 20000)])
 def test_subm_conv_bench_tile_configs_vs_oracle(Cin, Cout, n_rows, conv_kernel):
-    """The tile configurations the 150k-point bench actually runs (>= 148 row tiles, so no column shrink / split-K of
-    the small cases above): compared with the float64-accumulating oracle PER ELEMENT at the north-star tolerance."""
+    """The tile configurations the 150k-point bench actually runs (>= 148 row tiles, more than the 132 SMs of an H100, so
+    no column shrink / split-K of the small cases above): compared with the float64-accumulating oracle PER ELEMENT at the
+    north-star tolerance."""
     idx = _surface_case(Cin * 7 + Cout, n_rows)
     rng = np.random.RandomState(Cin + Cout)
     feats = (rng.randn(len(idx), Cin) * rng.uniform(0.2, 3.0, size=(1, Cin))).astype(np.float32)
@@ -253,7 +255,7 @@ def test_plan_equals_module_path(channels, num_blocks, n):
 
 
 def test_both_conv_kernels_bit_identical_and_choice():
-    """The two tcgen05 kernels evaluate the same products in the same order: bit-identical rows at a bench-size level
+    """The two launches evaluate the same products in the same order: bit-identical rows at a bench-size level
     (residual + bias + packed twin output), and sgb_spconv_kernel_choice follows the documented rule."""
     from softgroup_b200.ops import _lib
     from softgroup_b200.spconv import core

@@ -1,17 +1,14 @@
-"""CPU: the module tree / state_dict contract. When the reference tree is present (build container only),
-the UNMODIFIED reference SoftGroup class is instantiated on top of this repo's spconv/ops shims and its
-state_dict keys and shapes must equal ours one to one (checkpoints load unchanged, softgroup/util/utils.py:111-145)."""
+"""CPU: the module tree / state_dict contract. The UNMODIFIED reference SoftGroup class, instantiated on top of this
+repo's spconv/ops shims, has state_dict keys and shapes equal to ours one to one (checkpoints load unchanged,
+softgroup/util/utils.py:111-145)."""
+import json
 import os
-import sys
 
 import pytest
 import torch
 
 from softgroup_b200.configs import model_cfg
 from softgroup_b200.model import SoftGroup
-
-REF = '/root/reference'
-
 
 def test_state_dict_names():
     m = SoftGroup(**model_cfg('scannet'))
@@ -29,30 +26,18 @@ def test_state_dict_names():
     assert n_subm == 53 + 12  # backbone + tiny U-Net
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='reference tree only exists in the build container')
 def test_reference_class_on_our_shims_has_identical_state_dict():
-    import importlib
-    import types
-    import softgroup_b200
-    softgroup_b200.install_as_reference_backends()
-    # load the reference's model package without importing softgroup/__init__ side effects
-    pkg = types.ModuleType('softgroup')
-    pkg.__path__ = [os.path.join(REF, 'softgroup')]
-    sys.modules.setdefault('softgroup', pkg)
-    util = types.ModuleType('softgroup.util')
-    from softgroup_b200 import util as our_util
-    for n in ('cuda_cast', 'force_fp32', 'rle_decode', 'rle_encode'):
-        setattr(util, n, getattr(our_util, n))
-    sys.modules.setdefault('softgroup.util', util)
-    ref_model = importlib.import_module('softgroup.model.softgroup')
-    cfg = model_cfg('scannet')
-    ref = ref_model.SoftGroup(**cfg)
-    ours = SoftGroup(**cfg)
-    a, b = ref.state_dict(), ours.state_dict()
-    assert list(a.keys()) == list(b.keys())
-    for k in a:
-        assert a[k].shape == b[k].shape, k
-    ours.load_state_dict(a)  # strict
+    """The names and shapes, in order, of the state_dict of the UNMODIFIED reference SoftGroup(scannet) class built on
+    this repo's shims (tests/golden/ref_model_meta.json, tests/golden/make_reference_golden.py) equal ours, and a state
+    dict of that layout loads strictly."""
+    meta = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_model_meta.json')))
+    ref = meta['state_dict_scannet']
+    ours = SoftGroup(**model_cfg('scannet'))
+    b = ours.state_dict()
+    assert [k for k, _ in ref] == list(b.keys())
+    for k, shape in ref:
+        assert list(b[k].shape) == shape, k
+    ours.load_state_dict({k: torch.zeros(shape, dtype=b[k].dtype) for k, shape in ref})  # strict
 
 
 def test_model_survives_deepcopy_and_pickle():
