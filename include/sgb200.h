@@ -219,7 +219,9 @@ int sgb_spconv_forward(const float *d_in, int in_stride, int in_off, const int32
  *     identity (K == 1: 1x1 conv / nn.Linear). Outputs, either or both: d_out fp32 rows (strided: concat buffers);
  *     d_pk_out packed rows at channel offset pk_coff (multiple of 8) after y = relu?(x * pk_scale[c] + pk_shift[c]) per
  *     OUTPUT channel c -- the NEXT layer's BatchNorm(eval)+ReLU folded into this producer (an intermediate with a single
- *     consumer never exists in fp32); pk_fill != 0 also zeroes the upper half of a last chunk that N leaves half written.
+ *     consumer never exists in fp32); pk_fill != 0 also zeroes channels [pk_coff + N, round_up32(pk_coff + N)), the rest
+ *     of the 32-channel chunk the written channels end in (N = Cout rounded up to 16; padding channels [pk_coff + Cout,
+ *     pk_coff + N) are always written as zero), for any pk_coff; channels below pk_coff are never written.
  *   sgb_act_pack: the same packing for tensors without a producing convolution (C real channels, zeros up to Cfill).
  *   sgb_spconv_overflow: a packed value beyond the fp16 range (|y| > 65504, or NaN) raises a per-device flag instead of
  *     saturating silently; this call reads and clears it (blocking 4-byte read on `stream`).

@@ -57,7 +57,7 @@ struct TcArgs {
   float *out; int out_stride, out_off;   // optional fp32 rows
   uint32_t *pk; int pk_stride, pk_coff;  // optional packed rows: row stride in words, first channel (multiple of 8)
   const float *pk_scale, *pk_shift; int pk_relu;  // per OUTPUT channel (nullptr: identity): the consumer's BatchNorm+ReLU
-  int pk_fill;                           // zero the rest of a half-written last 32-channel chunk
+  int pk_fill;                           // zero the rest of the 32-channel chunk the written channels end in
   int *oflow;                            // device flag: a packed value beyond the fp16 range
 };
 
@@ -280,13 +280,13 @@ __global__ void __launch_bounds__(TC_THREADS, tc_min_blocks<NT>()) spconv_tc_ker
             dst[16] = *reinterpret_cast<const uint32_t *>(&ll);
           }
         }
-        if (p.pk && p.pk_fill && n0 + nt == p.N && (p.N & 31)) {
-          // N = Cout rounded to 16 ends in the middle of a 32-channel chunk: the consumer reads whole chunks, so the
-          // upper 16 channels (8 words hi + 8 words lo) must be zero (not stale memory: 0 * NaN would poison the sums);
-          // the 4 threads of the row write 2 + 2 words each
+        if (p.pk && p.pk_fill && n0 + nt == p.N && ((p.pk_coff + p.N) & 31)) {
+          // the written channels end in the middle of a 32-channel chunk: the consumer reads whole chunks, so channels
+          // [pk_coff + N, round_up32(pk_coff + N)) -- 8, 16 or 24 of them, hi and lo words -- must be zero (not stale
+          // memory: 0 * NaN would poison the sums); the 4 threads of the row share the words
           const int ch2 = p.pk_coff + p.N;
-          uint32_t *zp = p.pk + (size_t)row * p.pk_stride + (ch2 >> 5) * 32 + ((ch2 & 31) >> 1) + cl;
-          zp[0] = 0u; zp[1] = 0u; zp[16] = 0u; zp[17] = 0u;
+          uint32_t *zp = p.pk + (size_t)row * p.pk_stride + (ch2 >> 5) * 32;
+          for (int w = ((ch2 & 31) >> 1) + (lane & 3); w < 16; w += 4) { zp[w] = 0u; zp[w + 16] = 0u; }
         }
       }
     }

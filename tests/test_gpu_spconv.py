@@ -260,12 +260,14 @@ def test_both_conv_kernels_bit_identical_and_choice():
     from softgroup_b200.ops import _lib
     from softgroup_b200.spconv import core
     L = _lib.lib()
-    assert L.sgb_spconv_kernel_choice(27, 137100, 32, 32, 148) == 1    # level 0: >= 4 * 148 row tiles
-    assert L.sgb_spconv_kernel_choice(27, 42391, 96, 96, 148) == 1     # level 2
-    assert L.sgb_spconv_kernel_choice(27, 1933, 160, 160, 148) == 1    # level 4: 16 row tiles is the threshold
-    assert L.sgb_spconv_kernel_choice(27, 1900, 160, 160, 148) == 0
-    assert L.sgb_spconv_kernel_choice(27, 332, 192, 192, 148) == 0     # deep level: split-K clusters
-    assert L.sgb_spconv_kernel_choice(27, 36000, 32, 32, 148) == 0     # 32-channel tiny U-Net
+    sms = torch.cuda.get_device_properties(0).multi_processor_count  # what the launch plans with (132 on H100 SXM5)
+    assert L.sgb_spconv_kernel_choice(27, 137100, 32, 32, sms) == 1    # level 0: >= 4 * sms row tiles
+    assert L.sgb_spconv_kernel_choice(27, 42391, 96, 96, sms) == 1     # level 2
+    assert L.sgb_spconv_kernel_choice(27, 1933, 160, 160, sms) == 1    # level 4: 16 row tiles is the threshold
+    assert L.sgb_spconv_kernel_choice(27, 1900, 160, 160, sms) == 0
+    assert L.sgb_spconv_kernel_choice(27, 332, 192, 192, sms) == 0     # deep level: split-K clusters
+    assert L.sgb_spconv_kernel_choice(27, 128 * (4 * sms - 1), 32, 32, sms) == 0  # 32-channel tiny U-Net: < 4 * sms tiles
+    assert L.sgb_spconv_kernel_choice(27, 128 * 4 * sms, 32, 32, sms) == 1
     idx = _surface_case(11, 30000)
     rng = np.random.RandomState(5)
     Cin, Cout = 96, 64
