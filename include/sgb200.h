@@ -143,7 +143,13 @@ int sgb_bfs_cluster_fill(const int32_t *d_ball_query_idxs, const int32_t *d_star
 /* ---------------------------------------------------------------------------------------------
  * Segment reductions -- replace sec_mean / sec_min / sec_max (sec_mean/sec_mean.cu:13-93) and
  * global_avg_pool_fp / _bp (roipool/roipool.cu:12-72). inp f32 [S,C]; offsets int32 [nP+1]; out f32 [nP,C].
- * min/max are exact; mean / avg-pool use a tree reduction (within 1e-5 rel of the sequential sums).
+ * Proposal p covers rows [offsets[p], offsets[p+1]); rows outside every proposal are never read.
+ * min/max are exact: every value equals the reference's (`<` / `>` scans: NaN never wins, an empty proposal gives
+ * +inf / -inf); only the sign of a zero result is not guaranteed, because the tree reduction cannot reproduce the
+ * reference's first-occurrence choice between +0.0 and -0.0. mean / avg-pool sum len/rows_par terms per thread, then a
+ * log2(rows_par) tree (rows_par = 256 / min(pow2 >= C, 32)), so per element
+ * |out - mean64| <= (ceil(len/rows_par) + log2(rows_par) + 2) * 2^-24 * sum|x| / len; an empty proposal gives 0 (mean) /
+ * NaN (avg-pool, 0/0).
  * ------------------------------------------------------------------------------------------- */
 int sgb_sec_mean(const float *d_inp, const int32_t *d_offsets, float *d_out, int nProposal, int C, void *stream);
 int sgb_sec_min(const float *d_inp, const int32_t *d_offsets, float *d_out, int nProposal, int C, void *stream);

@@ -7,7 +7,7 @@
 // 2048-row chunks spread over a machine-filling grid, a chunk is split at proposal boundaries, and the per-chunk partial
 // of every (proposal, channel) is combined with one atomic min/max on the sign-aware integer image of the float
 // (seg_minmax_kernel) -- 40 long proposals no longer mean 40 busy SMs. mean/avg: one CTA per proposal, shared-memory
-// tree (within 1e-6 relative of the reference's sequential sums).
+// tree (error bound in include/sgb200.h).
 #include <float.h>
 
 #include "common.cuh"
@@ -66,12 +66,17 @@ __global__ void __launch_bounds__(kSegThreads) seg_reduce_kernel(const float *__
 // ---- chunked min / max -------------------------------------------------------------------------------------------
 constexpr int kSegChunk = 2048;
 
+// The branch is chosen by the sign BIT, not by `v >= 0.f` (true for -0.0, whose int image is INT_MIN): floats with the
+// sign bit clear are ordered like their int images, floats with it set are ordered inversely to their unsigned images,
+// and every sign-clear image is below every sign-set one as unsigned and above it as signed. So a signed atomicMin /
+// atomicMax for sign-clear values and an unsigned atomicMax / atomicMin for sign-set values order any mix correctly
+// (-0.0 sorts just below +0.0, which only decides the sign of a zero result).
 __device__ __forceinline__ void atomic_min_f32(float *addr, float v) {  // *addr starts at +inf; NaN never gets here
-  if (v >= 0.f) atomicMin(reinterpret_cast<int *>(addr), __float_as_int(v));
+  if (__float_as_int(v) >= 0) atomicMin(reinterpret_cast<int *>(addr), __float_as_int(v));
   else atomicMax(reinterpret_cast<unsigned int *>(addr), __float_as_uint(v));
 }
 __device__ __forceinline__ void atomic_max_f32(float *addr, float v) {  // *addr starts at -inf
-  if (v >= 0.f) atomicMax(reinterpret_cast<int *>(addr), __float_as_int(v));
+  if (__float_as_int(v) >= 0) atomicMax(reinterpret_cast<int *>(addr), __float_as_int(v));
   else atomicMin(reinterpret_cast<unsigned int *>(addr), __float_as_uint(v));
 }
 
@@ -87,9 +92,10 @@ __global__ void __launch_bounds__(kSegThreads) seg_minmax_kernel(const float *__
   const int rows_par = kSegThreads / Cw;
   const int tx = threadIdx.x % Cw, ty = threadIdx.x / Cw;
   const int S = offsets[nProposal];
+  const int first = offsets[0];  // rows below offsets[0] belong to no proposal
   for (long long r0l = (long long)blockIdx.x * kSegChunk; r0l < S; r0l += (long long)gridDim.x * kSegChunk) {
-    int r0 = (int)r0l;
-    const int r1 = min(r0 + kSegChunk, S);
+    const int r1 = min((int)r0l + kSegChunk, S);
+    int r0 = max((int)r0l, first);
     // proposal holding row r0: last p with offsets[p] <= r0
     int lo = 0, hi = nProposal;
     while (hi - lo > 1) {
