@@ -329,19 +329,19 @@ int sgb_affine3_f64(const float *d_xyz, const double *h_m9, double *d_out, int N
 
 
 /* ---------------------------------------------------------------------------------------------
- * Sparse U-Net executor (unet.cu): one backbone pass = ONE call. The plan (array of sgb_unet_op) is compiled once per
- * model by softgroup_b200/model/unet_plan.py from the module tree of softgroup/model/blocks.py:44-143 with the fusion the
- * module path applies (consumer BatchNorm+ReLU in the producer's epilogue, packed activations, residual / concat writes in
+ * Sparse U-Net executor (unet.cu): runs n_ops records of a plan in one call. The plan (array of sgb_unet_op) is compiled
+ * once per model by softgroup_b200/model/unet_plan.py from the module tree of softgroup/model/blocks.py:44-143, fused
+ * across modules (consumer BatchNorm+ReLU in the producer's epilogue, packed activations, residual / concat writes in
  * epilogues); per scan the caller supplies row counts M[level], rulebooks per level (subm [27][M_l], down [8][M_{l+1}],
- * inverse [8][M_l]) and one pointer per plan buffer. Results are those of the same launches issued one by one.
+ * inverse [8][M_l]) and one pointer per plan buffer. Results do not depend on how the ops are split into calls.
  * ------------------------------------------------------------------------------------------- */
-enum { SGB_UNET_CONV = 1, SGB_UNET_ACT_PACK = 2, SGB_UNET_COPY_COLS = 3, SGB_UNET_BN_RELU = 4 };
+enum { SGB_UNET_CONV = 1, SGB_UNET_ACT_PACK = 2, SGB_UNET_BN_RELU = 4 };
 typedef struct sgb_unet_op {
   int32_t kind;                     /* SGB_UNET_* */
   int32_t level_in, level_out;      /* rows of the input / output: M[level] */
   int32_t map_kind;                 /* CONV: 0 identity (K = 1), 1 subm of level_out, 2 down level_in -> level_in + 1, 3 inverse -> level_out */
-  int32_t K, Cin, Cout;             /* ACT_PACK: Cin = real channels, Cout = fill width; COPY / BN_RELU: Cin = channels */
-  int32_t in_buf, in_stride, in_off;          /* fp32 source (ACT_PACK, COPY_COLS, BN_RELU) */
+  int32_t K, Cin, Cout;             /* ACT_PACK: Cin = real channels, Cout = fill width; BN_RELU: Cin = channels */
+  int32_t in_buf, in_stride, in_off;          /* fp32 source (ACT_PACK, BN_RELU) */
   int32_t pk_in_buf, pk_in_stride;            /* CONV: packed input, row stride in words */
   int32_t out_buf, out_stride, out_off;       /* fp32 destination (-1: none) */
   int32_t pk_out_buf, pk_out_stride, pk_out_coff, pk_fill, relu;  /* packed destination (-1: none) */

@@ -2,22 +2,11 @@
 // from ONE C call instead of ~170 Python->ctypes round trips (the host side of the forward was the bottleneck once the
 // kernels got faster: Python spent longer per convolution than the GPU).
 // The plan is data: softgroup_b200/model/unet_plan.py walks the module tree of the reference-shaped model
-// (softgroup/model/blocks.py:44-143 -- ResidualBlock / UBlock) once and emits one record per launch, with the same fusion
-// decisions as the module path (BatchNorm+ReLU of the consumer folded into the producing conv's epilogue, packed
-// activations between convs, residual adds and concat writes in the epilogues). Per scan only the row counts, the
-// rulebook pointers and the buffer pointers change.
+// (softgroup/model/blocks.py:44-143 -- ResidualBlock / UBlock) once and emits one record per launch, fused across modules
+// (BatchNorm+ReLU of the consumer folded into the producing conv's epilogue, packed activations between convs, residual
+// adds and concat writes in the epilogues). Per scan only the row counts, the rulebook pointers and the buffer pointers
+// change. The caller runs a segment of ops per call, or one op per call when it times each launch.
 #include "common.cuh"
-
-namespace sgb {
-__global__ void copy_cols_kernel(const float *__restrict__ src, int s_stride, int s_off, float *__restrict__ dst, int d_stride,
-                                 int d_off, int M, int C4) {
-  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= (long long)M * C4) return;
-  const int row = (int)(t / C4), c = (int)(t % C4);
-  reinterpret_cast<float4 *>(dst + (size_t)row * d_stride + d_off)[c] =
-      __ldg(reinterpret_cast<const float4 *>(src + (size_t)row * s_stride + s_off) + c);
-}
-}  // namespace sgb
 
 extern "C" int sgb_unet_run(const sgb_unet_op *ops, int n_ops, float *const *bufs, const int32_t *const *subm_maps,
                             const int32_t *const *down_maps, const int32_t *const *inv_maps, const int *M, int n_levels,
@@ -52,17 +41,6 @@ extern "C" int sgb_unet_run(const sgb_unet_op *ops, int n_ops, float *const *buf
         rc = sgb_bn_relu(bufs[o.in_buf] + o.in_off, o.in_stride, o.scale, o.shift, o.relu, bufs[o.out_buf] + o.out_off, o.out_stride,
                          Min, o.Cin, stream);
         break;
-      case SGB_UNET_COPY_COLS: {
-        if (Min == 0) break;
-        SGB_REQUIRE((o.Cin & 3) == 0 && (o.in_stride & 3) == 0 && (o.in_off & 3) == 0 && (o.out_stride & 3) == 0 && (o.out_off & 3) == 0,
-                    SGB_ERR_ARG, "unet_run: copy needs multiples of 4 floats");
-        const long long tot = (long long)Min * (o.Cin / 4);
-        sgb::copy_cols_kernel<<<sgb::div_up(tot, 256), 256, 0, (cudaStream_t)stream>>>(bufs[o.in_buf], o.in_stride, o.in_off,
-                                                                                     bufs[o.out_buf], o.out_stride, o.out_off, Min,
-                                                                                     o.Cin / 4);
-        SGB_LAUNCH_CHECK();
-        break;
-      }
       default:
         SGB_REQUIRE(false, SGB_ERR_ARG, "unet_run: unknown op kind");
     }

@@ -6,6 +6,9 @@ What changes underneath (results equal within fp32 rounding):
   * the residual add of ResidualBlock is the second conv's epilogue;
   * the decoder's SparseInverseConv3d writes straight into the right half of the [M, 2C] concat buffer;
   * MLP heads run through the same kernel (K=1 identity map) with bias / BN / ReLU fused.
+
+Each block packs its own input here. On the tensor-core path SoftGroup runs the U-Net as a compiled plan instead
+(model/unet_plan.py), which fuses across blocks too; both give bit-identical features.
 """
 from collections import OrderedDict
 
@@ -106,18 +109,10 @@ class ResidualBlock(SparseModule):
             spconv.SubMConv3d(out_channels, out_channels, kernel_size=3, padding=1, bias=False,
                               indice_key=indice_key))
 
-    takes_next_act = True  # SparseSequential chains blocks: forward(input, next_act=<BatchNorm that consumes the output>)
-
-    def first_norm(self):
-        """The BatchNorm (followed by ReLU and a conv) that consumes this block's INPUT."""
-        return self.conv_branch[0]
-
-    def forward(self, input, next_act=None):
-        identity = spconv.SparseConvTensor(input.features, input.indices, input.spatial_shape, input.batch_size,
-                                           input.grid, input.indice_dict)
-        skip = self.i_branch(identity).features
+    def forward(self, input):
+        skip = self.i_branch(input).features
         # output.features + i_branch(identity).features (blocks.py:75-76), as the second conv's epilogue
-        return self.conv_branch(input, residual=skip, next_act=next_act)
+        return self.conv_branch(input, residual=skip)
 
 
 class UBlock(nn.Module):
@@ -146,38 +141,15 @@ class UBlock(nn.Module):
                                                          indice_key='subm{}'.format(indice_key_id))
             self.blocks_tail = spconv.SparseSequential(OrderedDict(blocks_tail))
 
-    takes_next_act = True
-
-    def first_norm(self):
-        return self.blocks[0].first_norm()
-
-    def forward(self, input, next_act=None):
-        deeper = len(self.nPlanes) > 1
-        fused = spconv.core.CONV_IMPL == 'tc' and input.features.is_cuda
-        # consumer of the encoder blocks' output: the BatchNorm in front of the strided conv (deeper) or our caller's
-        output = self.blocks(input, next_act=(self.conv[0] if deeper else next_act) if fused else None)
-        if deeper:
+    def forward(self, input):
+        output = self.blocks(input)
+        if len(self.nPlanes) > 1:
             C = self.nPlanes[0]
             M = output.features.size(0)
             # torch.cat((identity.features, output_decoder.features), dim=1) (blocks.py:140) without the cat:
             cat = torch.empty((M, 2 * C), dtype=output.features.dtype, device=output.features.device)
             cat[:, :C] = output.features
-            if not fused:
-                output_decoder = self.conv(output)
-                output_decoder = self.u(output_decoder)
-                self.deconv(output_decoder, out=cat, out_stride=2 * C, out_off=C)
-                output = output.replace_feature(cat)
-                return self.blocks_tail(output)
-            # packed twin of the concat buffer under the BatchNorm(2C)+ReLU of the first tail block: the left half comes
-            # from the encoder output (one pack pass), the right half is written by the inverse conv's epilogue
-            tail_bn = self.blocks_tail[0].first_norm()
-            ts, tb = fold_bn(tail_bn)
-            pk_cat = torch.empty((M, (2 * C + 31) // 32 * 32), dtype=torch.float32, device=cat.device)
-            spconv.core.act_pack(output.features, output.features.stride(0), 0, C, act=(ts[:C], tb[:C]), out=pk_cat, out_coff=0)
-            output_decoder = self.conv(output, next_act=self.u.first_norm())
-            output_decoder = self.u(output_decoder, next_act=self.deconv[0])
-            self.deconv(output_decoder, out=cat, out_stride=2 * C, out_off=C, emit_buf=(pk_cat, C, ts[C:], tb[C:], tail_bn))
-            output = output.replace_feature(cat)
-            output.packed[tail_bn] = pk_cat
-            output = self.blocks_tail(output, next_act=next_act)
+            output_decoder = self.u(self.conv(output))
+            self.deconv(output_decoder, out=cat, out_stride=2 * C, out_off=C)
+            output = self.blocks_tail(output.replace_feature(cat))
         return output

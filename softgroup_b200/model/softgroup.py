@@ -151,8 +151,8 @@ class SoftGroup(nn.Module):
             mod = getattr(self, mod)
             for param in mod.parameters():
                 param.requires_grad = False
-        # the backbone and the tiny U-Net run as compiled launch plans through ONE C call each (model/unet_plan.py); False =
-        # the module path, one ctypes call per launch (same kernels, same results; used for per-kernel instrumentation)
+        # the backbone and the tiny U-Net run as compiled launch plans, one C call per U-Net level (model/unet_plan.py);
+        # False = the same plan one launch per call, each in its own profiler record (per-kernel instrumentation)
         self.use_plan = True
         self._plans = {}
         self.stage_ms = None  # filled when profile_stages is set
@@ -344,18 +344,17 @@ class SoftGroup(nn.Module):
         return super().load_state_dict(*args, **kwargs)
 
     def _run_stack(self, name, input_conv, unet, output_layer, x):
-        """input_conv -> unet -> output_layer on SparseConvTensor x -> fp32 feature rows. Compiled plan (one C call) when
-        use_plan is set and the tensor path applies, else the module path."""
+        """input_conv -> unet -> output_layer on SparseConvTensor x -> fp32 feature rows. The compiled plan wherever the
+        tensor path applies (one C call per U-Net level, or one per launch when use_plan is False), else the module path."""
         from ..spconv import core
-        if (self.use_plan and core.CONV_IMPL == 'tc' and x.features.is_cuda and not self.training and
-                max(unet.nPlanes) <= 256):
+        if core.CONV_IMPL == 'tc' and x.features.is_cuda and not self.training and max(unet.nPlanes) <= 256:
             ver = self._weights_version()
             hit = self._plans.get(name)
             if hit is None or hit[0] != ver:
                 from .unet_plan import compile_backbone
                 hit = (ver, compile_backbone(input_conv, unet, output_layer))
                 self._plans[name] = hit
-            return hit[1].run(x)
+            return hit[1].run(x, per_launch=not self.use_plan)
         out = x
         if input_conv is not None:
             out = input_conv(out)

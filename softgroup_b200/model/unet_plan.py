@@ -3,7 +3,7 @@
 The module path (softgroup_b200/spconv/core.py SparseSequential + model/blocks.py) issues one ctypes call per launch:
 ~170 per backbone pass at ~40 us of Python each -- more than the GPU needs for most of them. `compile_backbone` walks the
 same module tree ONCE (input conv softgroup.py:60-61, UBlock / ResidualBlock blocks.py:44-143, output layer
-softgroup.py:65) and emits one `sgb_unet_op` record per launch with the SAME fusion decisions as the module path:
+softgroup.py:65) and emits one `sgb_unet_op` record per launch. It is the one place that fuses ACROSS modules:
 
   * activations travel packed (fp16 hi/lo) between convolutions; a conv whose output feeds BatchNorm+ReLU+conv writes
     that consumer's packed input from its epilogue (conv1 of a block writes no fp32 rows at all);
@@ -11,12 +11,16 @@ softgroup.py:65) and emits one `sgb_unet_op` record per launch with the SAME fus
     of the concat buffer, the inverse conv into the right half (fp32 and packed twins);
   * the 1x1 skip of the first tail block reads the raw concat buffer (one pack pass).
 
+The module path fuses only inside a SparseSequential and packs each block's input with a separate act_pack. That pass
+applies the same fmaxf(fmaf(y, scale, shift), 0) to the same fp32 rows as a conv epilogue, so both paths give
+bit-identical features (tests/test_gpu_spconv.py::test_plan_equals_module_path).
+
 Per scan `Plan.run` walks the plan in SEGMENTS, one `sgb_unet_run` call each (7 + 1 for the seven-level backbone): a
 segment ends where the next launch needs a U-Net level whose rulebook does not exist yet. Opening a level costs one host
 wait (the parent count of the strided rulebook); it is taken right after the previous segment's convolutions were enqueued,
-so the GPU keeps working through it. One arena per level holds that level's intermediate buffers. The launches are the
-same kernels with the same arguments as the module path, so the result is bit-identical to it
-(tests/test_gpu_spconv.py::test_plan_equals_module_path).
+so the GPU keeps working through it. One arena per level holds that level's intermediate buffers. `per_launch=True` runs
+the same ops one `sgb_unet_run` call each, inside a profiler record named like the module path's launch
+(`spconv_tc_kernel`, `act_pack`, `bn_relu`): the per-op timing of exactly the launches the segmented run makes.
 """
 import ctypes
 
@@ -29,7 +33,7 @@ from ..ops._lib import check
 from ..spconv import core
 from ..spconv.core import fold_bn
 
-CONV, ACT_PACK, COPY_COLS, BN_RELU = 1, 2, 3, 4
+CONV, ACT_PACK, BN_RELU = 1, 2, 4
 
 
 class UnetOp(ctypes.Structure):
@@ -92,10 +96,7 @@ class Plan(object):
             relu = bn is not None
         if into is None:
             into = self.new_buf(level, _r32(x.C))
-            fill = _r32(x.C)
-        else:
-            width = self.bufs[into][1]
-            fill = min(width - coff, _r32(x.C)) if (coff + x.C) % 32 else x.C
+        fill = core.pack_fill(x.C, self.bufs[into][1], coff)
         self.op(kind=ACT_PACK, level_in=level, level_out=level, Cin=x.C, Cout=fill, in_buf=x.buf, in_stride=x.stride, in_off=x.off,
                 pk_out_buf=into, pk_out_stride=self.bufs[into][1], pk_out_coff=coff, relu=int(bool(relu)), scale=self._dev(scale),
                 shift=self._dev(shift))
@@ -144,8 +145,18 @@ class Plan(object):
                 start, opened = i, need
         self.segments.append((start, len(self.ops), opened))
 
-    def run(self, x):
-        """x: SparseConvTensor (fp32 features [M0, Cin]) -> fp32 features [M0, Cout] of the compiled stack."""
+    @staticmethod
+    def _record_of(d, M):
+        """(profiler name, algorithmic bytes) of op `d` at the row counts M[level]."""
+        Min, Mout = M[d['level_in']], M[d['level_out']]
+        if d['kind'] == CONV:
+            name = 'spconv_tc_kernel' if d['map_kind'] else 'spconv_tc_kernel(1x1/linear)'
+            return name, core.conv_bytes(Min, Mout, d['K'], d['Cin'], d['Cout'], d['map_kind'] != 0, d['res_buf'] >= 0)
+        return ('act_pack' if d['kind'] == ACT_PACK else 'bn_relu'), 8 * Min * d['Cin']
+
+    def run(self, x, per_launch=False):
+        """x: SparseConvTensor (fp32 features [M0, Cin]) -> fp32 features [M0, Cout] of the compiled stack.
+        per_launch: one sgb_unet_run call and one profiler record per op instead of one call per segment."""
         assert self._c_ops is not None
         feats = x.features.contiguous()
         dev = feats.device
@@ -163,26 +174,12 @@ class Plan(object):
             if k == 0:
                 indices, shape = x.indices, x.spatial_shape
             else:
-                pidx, pshape = level_idx[k - 1]
-                key = self.key_of_level.get(k - 1, (None, None))[1]
-                rd = x.indice_dict.get(key) if key is not None else None
-                if rd is None:
-                    out_indices, mp, inv_mp, out_shape = core.build_down_map(pidx, pshape)
-                    rd = {'kind': 'down', 'map': mp, 'inv_map': inv_mp, 'out_indices': out_indices, 'out_shape': out_shape,
-                          'in_indices': pidx, 'in_shape': pshape}
-                    if key is not None:
-                        x.indice_dict[key] = rd
+                rd = core.rulebook(x.indice_dict, self.key_of_level.get(k - 1, (None, None))[1], 'down', *level_idx[k - 1])
                 down[k - 1], inv[k - 1] = rd['map'], rd['inv_map']
                 indices, shape = rd['out_indices'], rd['out_shape']
             level_idx[k] = (indices, shape)
             M[k] = indices.size(0)
-            key = self.key_of_level.get(k, (None, None))[0]
-            rb = x.indice_dict.get(key) if key is not None else None
-            if rb is None:
-                rb = {'kind': 'subm', 'map': core.build_subm_map(indices)}
-                if key is not None:
-                    x.indice_dict[key] = rb
-            subm[k] = rb['map']
+            subm[k] = core.rulebook(x.indice_dict, self.key_of_level.get(k, (None, None))[0], 'subm', indices)['map']
             total, offs = 0, []
             for b, width in bufs_of_level[k]:
                 offs.append(total)
@@ -217,9 +214,11 @@ class Plan(object):
                 if k > 0:
                     c_down[k - 1] = down[k - 1].data_ptr() if down[k - 1] is not None else None
                     c_inv[k - 1] = inv[k - 1].data_ptr() if inv[k - 1] is not None else None
-            seg = ctypes.cast(ctypes.byref(self._c_ops, i0 * op_size), ctypes.c_void_p)
-            with profiler.record('unet_run', 0):
-                check(lib.sgb_unet_run(seg, i1 - i0, c_bufs, c_subm, c_down, c_inv, c_M, L, stream), 'sgb_unet_run')
+            for j0, j1 in ([(i, i + 1) for i in range(i0, i1)] if per_launch else [(i0, i1)]):
+                name, nbytes = self._record_of(self.ops[j0], M) if per_launch else ('unet_run', 0)
+                seg = ctypes.cast(ctypes.byref(self._c_ops, j0 * op_size), ctypes.c_void_p)
+                with profiler.record(name, nbytes):
+                    check(lib.sgb_unet_run(seg, j1 - j0, c_bufs, c_subm, c_down, c_inv, c_M, L, stream), 'sgb_unet_run')
         o = self.out
         level, width = self.bufs[o.buf]
         base = ptrs[o.buf]

@@ -40,9 +40,6 @@ class SparseConvTensor(object):
         self.batch_size = batch_size
         self.indice_dict = indice_dict if indice_dict is not None else {}
         self.grid = grid
-        # packed (activated + fp16 hi/lo split) versions of `features`, keyed by the consumer BatchNorm module whose
-        # (scale, shift, ReLU) they were produced with; filled by producing convs (Emit), read by consuming convs
-        self.packed = {}
 
     def replace_feature(self, feature):
         out = SparseConvTensor(feature, self.indices, self.spatial_shape, self.batch_size, self.grid,
@@ -146,6 +143,23 @@ def build_down_map(indices, spatial_shape):
     return out_indices, mp, inv, [int(s) // 2 for s in spatial_shape]
 
 
+def rulebook(indice_dict, key, kind, indices, spatial_shape=None):
+    """The rulebook of indice_key `key` over the sites `indices`, built on first use and shared through `indice_dict`.
+    kind 'subm': {'map'}; kind 'down' (k2 s2, and its inverse): {'map', 'inv_map', 'out_indices', 'out_shape',
+    'in_indices', 'in_shape'}."""
+    rb = indice_dict.get(key) if key is not None else None
+    if rb is None:
+        if kind == 'subm':
+            rb = {'kind': 'subm', 'map': build_subm_map(indices)}
+        else:
+            out_indices, mp, inv, out_shape = build_down_map(indices, spatial_shape)
+            rb = {'kind': 'down', 'map': mp, 'inv_map': inv, 'out_indices': out_indices, 'out_shape': out_shape,
+                  'in_indices': indices, 'in_shape': spatial_shape}
+        if key is not None:
+            indice_dict[key] = rb
+    return rb
+
+
 CONV_IMPL = os.environ.get('SGB_CONV_IMPL', 'tc')  # 'tc' = wgmma tensor cores (default), 'ffma' = CUDA-core fp32 (A/B only)
 # which of the two launches of the tensor-core kernel the module path asks for: -1 = the library chooses (sgb_spconv_kernel_choice), 0 = register
 # gather, 1 = persistent shared-memory ring. Parity tests run every case under 0 and 1; the compiled plan always uses -1.
@@ -183,6 +197,12 @@ class WeightPack(object):
         return self.packed
 
 
+def pack_fill(C, width, coff):
+    """Channels sgb_act_pack writes when it packs C channels at channel `coff` of a packed buffer `width` channels wide:
+    C when they end on a 32-channel boundary, else C rounded up to 32, the rest zeroed (never past `width`)."""
+    return min(width - coff, (C + 31) // 32 * 32) if (coff + C) % 32 else C
+
+
 def act_pack(feats, in_stride, in_off, C, act=None, relu=None, out=None, out_coff=0, rows=None):
     """fp32 rows -> packed rows (per 32-channel chunk: 16 words fp16 hi pairs | 16 words lo pairs) after the optional
     BatchNorm(eval) `act = (scale, shift)` and ReLU. `out`: an existing packed buffer [M, cpad] float32-typed (concat
@@ -191,12 +211,9 @@ def act_pack(feats, in_stride, in_off, C, act=None, relu=None, out=None, out_cof
     if relu is None:
         relu = act is not None
     if out is None:
-        cpad = (C + 31) // 32 * 32
-        out = torch.empty((M, cpad), dtype=torch.float32, device=feats.device)
-        fill = cpad
-    else:
-        cpad = out.size(1)
-        fill = min(cpad - out_coff, (C + 31) // 32 * 32) if (out_coff + C) % 32 else C
+        out = torch.empty((M, (C + 31) // 32 * 32), dtype=torch.float32, device=feats.device)
+    cpad = out.size(1)
+    fill = pack_fill(C, cpad, out_coff)
     scale, shift = act if act is not None else (None, None)
     with profiler.record('act_pack', 8 * M * C):
         check(_lib.lib().sgb_act_pack(ptr(feats), in_stride, in_off, ptr(scale), ptr(shift), int(bool(relu)), ptr(out),
@@ -220,12 +237,20 @@ def check_overflow():
 class Emit(object):
     """What a producing conv writes besides (or instead of) fp32 rows: the packed rows of ITS CONSUMER's input, i.e.
     relu(y * scale + shift) split into fp16 hi/lo -- the consumer's BatchNorm(eval)+ReLU folded into this epilogue.
-    key: the consumer's BatchNorm module (identity of the activation); buf/coff: existing packed buffer + channel offset
-    (concat halves) or None for a fresh one; fill: zero the unused half of a last 32-channel chunk."""
-    __slots__ = ('scale', 'shift', 'key', 'buf', 'coff', 'fill')
+    buf/coff: existing packed buffer + channel offset (concat halves) or None for a fresh one (conv_forward stores it
+    here); fill: zero the unused half of a last 32-channel chunk. `key` is accepted so that existing callers keep working,
+    and is not used."""
+    __slots__ = ('scale', 'shift', 'buf', 'coff', 'fill')
 
-    def __init__(self, scale, shift, key, buf=None, coff=0, fill=True):
-        self.scale, self.shift, self.key, self.buf, self.coff, self.fill = scale, shift, key, buf, coff, fill
+    def __init__(self, scale, shift, key=None, buf=None, coff=0, fill=True):
+        self.scale, self.shift, self.buf, self.coff, self.fill = scale, shift, buf, coff, fill
+
+
+def conv_bytes(m_in, Mout, K, Cin, Cout, has_map, has_residual):
+    """Algorithmic bytes of one sparse convolution (SURVEY.md 8d): input rows once + weights + map + output rows
+    (+ residual rows)."""
+    return (4 * m_in * Cin + 4 * K * Cin * Cout + (4 * K * Mout if has_map else 0) + 4 * Mout * Cout +
+            (4 * Mout * Cout if has_residual else 0))
 
 
 def conv_forward(feats, in_stride, in_off, mp, K, Mout, W, Cin, Cout, act=None, residual=None, bias=None, out=None,
@@ -244,12 +269,9 @@ def conv_forward(feats, in_stride, in_off, mp, K, Mout, W, Cin, Cout, act=None, 
         out_stride = Cout
     scale, shift = act if act is not None else (None, None)
     rs, ro = (residual.stride(0), 0) if residual is not None else (0, 0)
-    # algorithmic bytes (SURVEY.md 8d): input rows once + weights + map + output rows (+ residual)
     if m_in is None:
         m_in = feats.size(0)
-    nbytes = 4 * m_in * Cin + 4 * K * Cin * Cout + (4 * K * Mout if mp is not None else 0) + 4 * Mout * Cout
-    if residual is not None:
-        nbytes += 4 * Mout * Cout
+    nbytes = conv_bytes(m_in, Mout, K, Cin, Cout, mp is not None, residual is not None)
     name = ('spconv_tc_kernel' if fused else 'spconv_kernel') + ('' if mp is not None else '(1x1/linear)')
     if fused:
         pk = packed_in if packed_in is not None else act_pack(feats, in_stride, in_off, Cin, act=act, relu=act is not None)
@@ -328,12 +350,9 @@ def _stride0(f):
 
 
 def _wrap(t, o, fuse):
-    """conv_forward result -> SparseConvTensor: fp32 rows (possibly None) + the packed rows emitted for the consumer."""
-    emit = fuse.get('emit') if fuse else None
-    if emit is not None:
-        o, pk = o
-        t.packed[emit.key] = pk
-    t.features = o
+    """conv_forward result -> SparseConvTensor of the fp32 rows (None when the conv wrote only the packed rows of its
+    consumer; those are in fuse['emit'].buf)."""
+    t.features = o[0] if fuse.get('emit') is not None else o
     return t
 
 
@@ -343,11 +362,7 @@ class SubMConv3d(_SparseConvBase):
     def forward(self, x, act=None, residual=None, out=None, out_stride=None, out_off=0, **fuse):
         assert self.kernel_size == [3, 3, 3], 'only the k=3 submanifold conv of the reference is built'
         f = self._features(x, fuse)
-        rb = x.find_indice_pair(self.indice_key)
-        if rb is None:
-            rb = {'kind': 'subm', 'map': build_subm_map(x.indices)}
-            if self.indice_key is not None:
-                x.indice_dict[self.indice_key] = rb
+        rb = rulebook(x.indice_dict, self.indice_key, 'subm', x.indices)
         M = x.indices.size(0)
         o = conv_forward(f, _stride0(f), 0, rb['map'], 27, M, self.weight_kio(), self.in_channels, self.out_channels,
                          act=act, residual=residual, bias=self.bias, out=out, out_stride=out_stride, out_off=out_off,
@@ -368,13 +383,7 @@ class SparseConv3d(_SparseConvBase):
             return _wrap(x.replace_feature(None), o, fuse)
         assert self.kernel_size == [2, 2, 2] and self.stride == [2, 2, 2] and self.padding == [0, 0, 0], \
             'only the k2 s2 p0 strided conv of the reference is built'
-        rb = x.find_indice_pair(self.indice_key)
-        if rb is None:
-            out_indices, mp, inv, out_shape = build_down_map(x.indices, x.spatial_shape)
-            rb = {'kind': 'down', 'map': mp, 'inv_map': inv, 'out_indices': out_indices, 'out_shape': out_shape,
-                  'in_indices': x.indices, 'in_shape': x.spatial_shape}
-            if self.indice_key is not None:
-                x.indice_dict[self.indice_key] = rb
+        rb = rulebook(x.indice_dict, self.indice_key, 'down', x.indices, x.spatial_shape)
         Mout = rb['out_indices'].size(0)
         o = conv_forward(f, _stride0(f), 0, rb['map'], 8, Mout, self.weight_kio(), self.in_channels, self.out_channels,
                          act=act, residual=residual, bias=self.bias, out=out, out_stride=out_stride, out_off=out_off,
@@ -445,25 +454,22 @@ class SparseSequential(SparseModule):
 
     @staticmethod
     def _flush(x, pending):
-        scale, shift, relu = pending[:3]
+        scale, shift, relu = pending
         if isinstance(x, SparseConvTensor):
             return x.replace_feature(bn_relu_rows(x.features, scale, shift, relu))
         return bn_relu_rows(x, scale, shift, relu)
 
-    def forward(self, input, residual=None, out=None, out_stride=None, out_off=0, next_act=None, emit_buf=None):
+    def forward(self, input, residual=None, out=None, out_stride=None, out_off=0):
         """residual / out* apply to the LAST sparse conv of the sequence (fused epilogue).
 
-        Tensor-core path: activations travel PACKED between convolutions. A conv followed inside this
-        sequence by BatchNorm+ReLU+conv writes only the packed rows its successor reads (that BatchNorm+ReLU folded into
-        its epilogue, no fp32 rows at all); `next_act` = the BatchNorm module that will consume this sequence's OUTPUT
-        (behind a ReLU, in front of a conv) makes the last conv emit those packed rows next to its fp32 rows, into
-        `emit_buf` = (packed buffer, channel offset, scale, shift) when the consumer reads a concat buffer. Child
-        modules that take the same hint (ResidualBlock) are chained the same way."""
+        Tensor-core path: a conv followed inside this sequence by BatchNorm+ReLU+conv writes only the packed rows its
+        successor reads (that BatchNorm+ReLU folded into its epilogue, no fp32 rows at all). Fusion across modules is the
+        compiled plan's (model/unet_plan.py)."""
         mods = list(self._modules.values())
         conv_idx = [i for i, m in enumerate(mods) if _takes_fusion(m)]
         last_conv = conv_idx[-1] if conv_idx else -1
         fused = CONV_IMPL == 'tc'
-        pending = None  # (scale, shift, relu, bn module)
+        pending = None  # (scale, shift, relu)
         carry = None    # packed input prepared by the previous conv of this sequence for exactly `pending`
         x = input
         for i, m in enumerate(mods):
@@ -474,59 +480,40 @@ class SparseSequential(SparseModule):
                 if pending is not None:
                     x = self._flush(x, pending)
                 s, b = fold_bn(m)
-                pending = (s, b, False, m)
+                pending = (s, b, False)
                 continue
             if isinstance(m, nn.ReLU) and pending is not None and not pending[2]:
-                pending = (pending[0], pending[1], True, pending[3])
+                pending = (pending[0], pending[1], True)
                 continue
             if _takes_fusion(m):
                 act, fuse = None, {}
                 if pending is not None:
                     if pending[2]:
                         act = (pending[0], pending[1])
-                        if fused and is_sparse_in:
-                            pk = carry if carry is not None else x.packed.get(pending[3])
-                            if pk is not None:
-                                fuse['packed_in'] = pk
+                        if carry is not None:
+                            fuse['packed_in'] = carry
                     else:  # BN without ReLU in front of a conv: not fusable into the relu'd input transform
                         x = self._flush(x, pending)
                     pending = None
                 carry = None
-                if fused and is_sparse_in and m.out_channels <= 256 and m.in_channels <= 512:
-                    nxt = mods[i + 1:i + 4]
-                    if (len(nxt) == 3 and isinstance(nxt[0], nn.BatchNorm1d) and not nxt[0].training and
-                            isinstance(nxt[1], nn.ReLU) and _takes_fusion(nxt[2]) and i != last_conv):
-                        es, eb = fold_bn(nxt[0])
-                        fuse['emit'] = Emit(es, eb, nxt[0])
-                        fuse['want_fp32'] = False  # the intermediate never leaves this sequence
-                    elif i == last_conv and emit_buf is not None:
-                        buf, coff, es, eb, key = emit_buf
-                        fuse['emit'] = Emit(es, eb, key, buf=buf, coff=coff, fill=False)
-                    elif i == last_conv and next_act is not None and i == len(mods) - 1:
-                        es, eb = fold_bn(next_act)
-                        fuse['emit'] = Emit(es, eb, next_act)
+                nxt = mods[i + 1:i + 4]
+                if (fused and is_sparse_in and m.out_channels <= 256 and m.in_channels <= 512 and i != last_conv and
+                        len(nxt) == 3 and isinstance(nxt[0], nn.BatchNorm1d) and not nxt[0].training and
+                        isinstance(nxt[1], nn.ReLU) and _takes_fusion(nxt[2])):
+                    fuse['emit'] = Emit(*fold_bn(nxt[0]))
+                    fuse['want_fp32'] = False  # the intermediate never leaves this sequence
                 if i == last_conv:
                     x = m(x, act=act, residual=residual, out=out, out_stride=out_stride, out_off=out_off, **fuse)
                 else:
                     x = m(x, act=act, **fuse)
-                if 'emit' in fuse and not fuse.get('want_fp32', True):
-                    carry = x.packed[fuse['emit'].key]
+                if 'emit' in fuse:
+                    carry = fuse['emit'].buf
                 continue
             if pending is not None:
                 x = self._flush(x, pending)
                 pending = None
             if isinstance(m, SparseModule):
-                if fused and getattr(m, 'takes_next_act', False):
-                    # chain blocks: the consumer of this block's output is the first BatchNorm of the next block, or the
-                    # consumer named by our caller when this is the last module
-                    hint = None
-                    if i + 1 < len(mods) and getattr(mods[i + 1], 'takes_next_act', False):
-                        hint = mods[i + 1].first_norm()
-                    elif i == len(mods) - 1:
-                        hint = next_act
-                    x = m(x, next_act=hint)
-                else:
-                    x = m(x)
+                x = m(x)
             elif isinstance(x, SparseConvTensor):
                 if isinstance(m, nn.Identity):
                     continue

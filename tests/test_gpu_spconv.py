@@ -223,9 +223,10 @@ def test_backbone_vs_oracle(channels, num_blocks, shape, n):
 
 @pytest.mark.parametrize('channels,num_blocks,n', [(16, 4, 6000), (32, 7, 30000)])
 def test_plan_equals_module_path(channels, num_blocks, n):
-    """The compiled launch plan (model/unet_plan.py -> ONE sgb_unet_run call) issues the same kernels with the same
-    arguments as the module path (one ctypes call per launch): bit-identical features, for the backbone (input conv +
-    U-Net + output layer) and for the tiny U-Net of the instance branch (no input conv)."""
+    """The compiled launch plan (model/unet_plan.py, fused across modules) and the module path (fused inside each
+    SparseSequential only, every block's input packed by act_pack) give bit-identical features, for the backbone (input
+    conv + U-Net + output layer) and for the tiny U-Net of the instance branch (no input conv). The plan run one launch
+    per call (use_plan = False) is bit-identical to its segmented run."""
     import oracle
     torch.manual_seed(0)
     scan = synth.make_scan('c2_scannet', seed=1, n_points=n)
@@ -241,17 +242,26 @@ def test_plan_equals_module_path(channels, num_blocks, n):
         with torch.no_grad():
             return model._run_stack(name, ic, un, ol, x).clone()
 
+    def modules(ic, un, ol, f, idx, shape, bs):
+        x = spconv.SparseConvTensor(f, idx, shape, bs)
+        with torch.no_grad():
+            return ol(un(ic(x) if ic is not None else x)).features.clone()
+
     f, idx = _cuda(vfeats), _cuda(vc.astype(np.int32))
     a = run(True, 'backbone', model.input_conv, model.unet, model.output_layer, f, idx, scan['spatial_shape'], 1)
-    b = run(False, 'backbone', model.input_conv, model.unet, model.output_layer, f, idx, scan['spatial_shape'], 1)
+    b = modules(model.input_conv, model.unet, model.output_layer, f, idx, scan['spatial_shape'], 1)
+    c = run(False, 'backbone', model.input_conv, model.unet, model.output_layer, f, idx, scan['spatial_shape'], 1)
     assert a.shape == b.shape and torch.equal(a, b)
+    assert torch.equal(a, c)
     # tiny U-Net on a 20^3 grid per "proposal" (clusters_voxelization output shape)
     rng = np.random.RandomState(3)
     occ = np.argwhere(rng.rand(5, 20, 20, 20) < 0.08).astype(np.int32)
     tf = torch.from_numpy(rng.randn(len(occ), channels).astype(np.float32)).cuda()
     a = run(True, 'tiny', None, model.tiny_unet, model.tiny_unet_outputlayer, tf, _cuda(occ), [20, 20, 20], 5)
-    b = run(False, 'tiny', None, model.tiny_unet, model.tiny_unet_outputlayer, tf, _cuda(occ), [20, 20, 20], 5)
+    b = modules(None, model.tiny_unet, model.tiny_unet_outputlayer, tf, _cuda(occ), [20, 20, 20], 5)
+    c = run(False, 'tiny', None, model.tiny_unet, model.tiny_unet_outputlayer, tf, _cuda(occ), [20, 20, 20], 5)
     assert torch.equal(a, b)
+    assert torch.equal(a, c)
 
 
 def test_both_conv_kernels_bit_identical_and_choice():
