@@ -262,11 +262,14 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
 /* ---------------------------------------------------------------------------------------------
  * Per-class point selection in front of the ball query, all classes in one pass (grouping.cu) -- replaces the loop body
  * softgroup/model/softgroup.py:430-446 (`(scores[:, class_id] > score_thr).nonzero()`, the `min_npoint` skip, the gathers
- * of batch_idxs / coords_float / pt_offsets) for the classes h_classes[0..nc) (host array, nc <= 32):
+ * of batch_idxs / coords_float / pt_offsets) for the classes h_classes[0..nc) (host array, any nc >= 1, ids in [0, C);
+ * N * nc and nc * B below 2^31):
  *   entries in class-major, ascending point order: d_pts[e] = point, d_seg[e] = rank(class) * B + batch_idxs[point],
  *   d_shifted[e] = coords[point] + offsets[point] (fp32), all with capacity N * nc; d_seg_offsets int32 [nc*B + 1] =
  *   first entry of every (class, batch item) segment; d_total int32 [1 + nc] = number of entries, then entries per class
- *   (0 for a class below min_npoint). d_scores = softmax scores [N][C]. No host synchronisation.
+ *   (0 for a class below min_npoint). d_scores = softmax scores [N][C]. No host synchronisation and no host-to-device
+ *   copy: the class ids travel in the kernel parameters, 256 per launch (4 launches up to 256 classes, one more per
+ *   further 256). The segments feed sgb_ballquery_batch_p_async, which takes at most 1023 of them: nc * B <= 1023 there.
  * ------------------------------------------------------------------------------------------- */
 size_t sgb_group_entries_workspace_bytes(int N, int nc, int B);
 int sgb_group_entries(const float *d_scores, int N, int C, const int *h_classes, int nc, float score_thr, int min_npoint,

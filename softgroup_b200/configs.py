@@ -67,10 +67,25 @@ _SCANNET_PP = dict(  # configs/softgroup++/softgroup++_scannet.yaml:1-36 (the on
                   eval_tasks=['semantic', 'instance']),
     fixed_modules=[])
 
-CONFIGS = {'scannet': _SCANNET, 's3dis': _S3DIS, 'kitti': _KITTI, 'stpls3d++': _STPLS3D_PP, 'scannet++': _SCANNET_PP}
+_SCANNET200 = dict(  # a custom dataset as docs/custom_dataset.md describes it: ScanNet200's 200 semantic classes (198 grouped)
+    # on the ScanNet model. The reference ships no such config: class_numpoint_mean is SYNTHETIC (log-spaced 500..10000
+    # points per instance), not measured on ScanNet200.
+    channels=32, num_blocks=7, semantic_classes=200, instance_classes=198, sem2ins_classes=[], semantic_only=False,
+    ignore_label=-100,
+    grouping_cfg=dict(score_thr=0.2, radius=0.04, mean_active=300,
+                      class_numpoint_mean=[-1., -1.] + [float(round(500 * 20 ** (k / 197))) for k in range(198)],
+                      npoint_thr=0.05, ignore_classes=[0, 1]),
+    instance_voxel_cfg=dict(scale=50, spatial_shape=20),
+    train_cfg=dict(max_proposal_num=200, pos_iou_thr=0.5),
+    test_cfg=dict(x4_split=False, cls_score_thr=0.001, mask_score_thr=-0.5, min_npoint=100,
+                  eval_tasks=['semantic', 'instance']),
+    fixed_modules=[])
+
+CONFIGS = {'scannet': _SCANNET, 's3dis': _S3DIS, 'kitti': _KITTI, 'stpls3d++': _STPLS3D_PP, 'scannet++': _SCANNET_PP,
+           'scannet200': _SCANNET200}
 # which synthetic shape (softgroup_b200.synth.SHAPES) goes with which config
 SHAPE_OF = {'scannet': 'c2_scannet', 's3dis': 'c3_s3dis', 'kitti': 'c4_kitti', 'stpls3d++': 'c5_stpls3d',
-            'scannet++': 'c2_scannet'}
+            'scannet++': 'c2_scannet', 'scannet200': 'c6_scannet200'}
 
 
 def model_cfg(name='scannet', **overrides):

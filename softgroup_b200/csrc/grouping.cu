@@ -11,156 +11,193 @@
 // the same thing was ~30 small launches (index, compare, sum, nonzero, bincount, cumsum, gathers) with two host
 // synchronisations and two pageable H2D copies in the middle of the forward; this is 4 launches and none.
 // Selection is a strict fp32 comparison on the caller's softmax scores: bit-exact by construction.
+//
+// Any number of classes (ScanNet200 groups 198): the selection is kept as one 32-bit word per (tile of 32 points, class
+// rank), written once by ge_count_kernel and read by ge_fill_kernel instead of the scores. ge_count_kernel reads the scores
+// with one class per lane, so every load instruction takes consecutive columns of one row whatever C is. The class ids
+// travel by value in the kernel parameters (GE_SLICE per launch; more classes take one more count launch per slice), so
+// there is no host wait and no host-to-device copy.
 #include <algorithm>
 
 #include "common.cuh"
 
 namespace sgb {
 
-constexpr int GE_THREADS = 256;  // one point per thread
-constexpr int GE_MAXC = 32;      // classes per call (one bit of a thread's selection mask each)
+constexpr int GE_THREADS = 256;               // a block: 256 points = GE_TILES tiles of 32 points, one warp each
+constexpr int GE_TILES = GE_THREADS / 32;
+constexpr int GE_SLICE = 256;                 // class ids per ge_count_kernel launch (1 KB of kernel parameters)
+constexpr int GE_SCAN_THREADS = 1024;
 
 struct GeArgs {
   const float *scores; int N, C;
-  int cls[GE_MAXC]; int nc;
+  int nc;
   float thr; int min_npoint;
   const int32_t *batch; int B;
   const float *coords, *offsets;
   int32_t *pts, *seg; float *shifted;
   int32_t *seg_offsets;   // [nc * B + 1]
-  int32_t *blk_cnt;       // [nc][nblk] counts, scanned in place to global entry offsets
+  uint32_t *sel;          // [nblk * GE_TILES][nc]: bit q of sel[t][j] = point 32t+q passes class rank j
+  int32_t *blk_cnt;       // [nblk][nc] counts, scanned in place to entry offsets within the class
   int32_t *seg_cnt;       // [nc * B]
   int32_t *total;         // [1 + nc]: entries, then kept count per class
   int nblk;
 };
 
-// counts per (class, block of 256 points)
-__global__ void ge_count_kernel(GeArgs p) {
-  __shared__ int s_cnt[GE_MAXC];
-  const int tid = threadIdx.x, lane = tid & 31;
-  if (tid < p.nc) s_cnt[tid] = 0;
-  __syncthreads();
-  const int pt = blockIdx.x * GE_THREADS + tid;
-  const float *row = p.scores + (size_t)min(pt, p.N - 1) * p.C;
-  for (int j = 0; j < p.nc; j++) {
-    const bool f = pt < p.N && row[p.cls[j]] > p.thr;
-    const unsigned int b = __ballot_sync(0xffffffffu, f);
-    if (lane == 0 && b) atomicAdd(&s_cnt[j], __popc(b));
+struct GeSlice {  // class ranks [j0, j0 + n) and their score columns
+  int j0, n;
+  int col[GE_SLICE];
+};
+
+__device__ __forceinline__ int warp_incl_scan(int x) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
   }
-  __syncthreads();
-  if (tid < p.nc) p.blk_cnt[(size_t)tid * p.nblk + blockIdx.x] = s_cnt[tid];
+  return x;
 }
 
-// one CTA: class totals -> keep (>= min_npoint) -> class bases -> per-(class, block) entry offsets in place
+// exclusive scan of v over the CTA, sum = the CTA's total; every thread calls it (s_part: 32 ints)
+__device__ __forceinline__ int block_excl_scan(int v, int *s_part, int &sum) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  const int x = warp_incl_scan(v);
+  if (lane == 31) s_part[warp] = x;
+  __syncthreads();
+  if (warp == 0) {
+    const int w = warp_incl_scan(lane < nw ? s_part[lane] : 0);
+    s_part[lane] = w;  // inclusive over warps
+  }
+  __syncthreads();
+  const int r = (warp ? s_part[warp - 1] : 0) + x - v;
+  sum = s_part[nw - 1];
+  __syncthreads();  // s_part is reused by the next call
+  return r;
+}
+
+// selection words and counts per (class, block of 256 points) for the class ranks of one slice. Lane l takes class rank
+// j0 + k0 + l and walks the 32 points of its warp's tile.
+__global__ void ge_count_kernel(GeArgs p, GeSlice s) {
+  __shared__ int s_cnt[GE_TILES][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int t = blockIdx.x * GE_TILES + warp;  // tile: points [32t, 32t + 32)
+  const int np = min(32, p.N - t * 32);        // <= 0 for the empty tiles of the last block
+  for (int k0 = 0; k0 < s.n; k0 += 32) {
+    const int r = k0 + lane;
+    const bool on = r < s.n;
+    uint32_t m = 0u;
+    if (on && np > 0) {
+      const float *col = p.scores + (size_t)t * 32 * p.C + s.col[r];
+      const size_t ld = p.C;
+#pragma unroll 1
+      for (int q0 = 0; q0 < 32; q0 += 16) {
+        float v[16];  // 16 loads in flight before the first compare (rows past N re-read the tile's last row)
+#pragma unroll
+        for (int q = 0; q < 16; q++) v[q] = __ldg(col + min(q0 + q, np - 1) * ld);
+#pragma unroll
+        for (int q = 0; q < 16; q++)
+          if (q0 + q < np && v[q] > p.thr) m |= 1u << (q0 + q);
+      }
+    }
+    if (on) p.sel[(size_t)t * p.nc + s.j0 + r] = m;
+    s_cnt[warp][lane] = __popc(m);
+    __syncthreads();
+    if (warp == 0 && on) {
+      int c = 0;
+#pragma unroll
+      for (int w = 0; w < GE_TILES; w++) c += s_cnt[w][lane];
+      p.blk_cnt[(size_t)blockIdx.x * p.nc + s.j0 + r] = c;
+    }
+    __syncthreads();
+  }
+}
+
+// one CTA per class rank j: its block counts -> entry offsets within the class (in place), the class total and the
+// `object_idxs.size(0) < min_npoint -> continue` drop; zeroes the class's segment counters for ge_fill_kernel
 __global__ void ge_scan_kernel(GeArgs p) {
-  __shared__ int s_tot[GE_MAXC], s_base[GE_MAXC];
   __shared__ int s_part[32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
-  for (int j = 0; j < p.nc; j++) {  // exclusive scan of class j's block counts (chunks of blockDim.x)
-    int run = 0;
-    int32_t *c = p.blk_cnt + (size_t)j * p.nblk;
-    for (int b0 = 0; b0 < p.nblk; b0 += blockDim.x) {
-      const int i = b0 + tid;
-      const int v = i < p.nblk ? c[i] : 0;
-      int x = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-      }
-      if (lane == 31) s_part[warp] = x;
-      __syncthreads();
-      if (warp == 0) {
-        int w = lane < nw ? s_part[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const int y = __shfl_up_sync(0xffffffffu, w, o);
-          if (lane >= o) w += y;
-        }
-        s_part[lane] = w;  // inclusive over warps
-      }
-      __syncthreads();
-      const int before = (warp ? s_part[warp - 1] : 0) + x - v;
-      if (i < p.nblk) c[i] = run + before;
-      run += s_part[nw - 1];
-      __syncthreads();
-    }
-    if (tid == 0) s_tot[j] = run;
+  const int j = blockIdx.x;
+  int run = 0;
+  for (int b0 = 0; b0 < p.nblk; b0 += blockDim.x) {
+    const int i = b0 + threadIdx.x;
+    const int v = i < p.nblk ? p.blk_cnt[(size_t)i * p.nc + j] : 0;
+    int sum;
+    const int e = block_excl_scan(v, s_part, sum);
+    if (i < p.nblk) p.blk_cnt[(size_t)i * p.nc + j] = run + e;
+    run += sum;
   }
-  __syncthreads();
-  if (tid == 0) {
-    int base = 0;
-    for (int j = 0; j < p.nc; j++) {
-      const bool keep = s_tot[j] >= p.min_npoint;  // `object_idxs.size(0) < min_npoint -> continue`
-      s_base[j] = keep ? base : -1;
-      p.total[1 + j] = keep ? s_tot[j] : 0;
-      if (keep) base += s_tot[j];
-    }
-    p.total[0] = base;
-  }
-  __syncthreads();
-  for (int j = 0; j < p.nc; j++) {
-    int32_t *c = p.blk_cnt + (size_t)j * p.nblk;
-    const int base = s_base[j];
-    for (int i = tid; i < p.nblk; i += blockDim.x) c[i] = base < 0 ? -1 : c[i] + base;
-  }
-  for (int i = tid; i < p.nc * p.B; i += blockDim.x) p.seg_cnt[i] = 0;
+  if (threadIdx.x == 0) p.total[1 + j] = run >= p.min_npoint ? run : 0;
+  for (int i = threadIdx.x; i < p.B; i += blockDim.x) p.seg_cnt[(size_t)j * p.B + i] = 0;
 }
 
+// ordered compaction, one point per lane: the entry of (class rank j, point) goes to the class base (exclusive scan of the
+// kept totals, recomputed per warp 32 classes at a time) + the block's offset in the class + the earlier tiles of the
+// block + the earlier lanes of the tile
 __global__ void ge_fill_kernel(GeArgs p) {
-  __shared__ int s_w[GE_THREADS / 32][GE_MAXC];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int pt = blockIdx.x * GE_THREADS + tid;
-  const bool in = pt < p.N;
-  const float *row = p.scores + (size_t)min(pt, p.N - 1) * p.C;
-  unsigned int mine = 0u;  // bit j: this point is selected for class j
-  for (int j = 0; j < p.nc; j++) {
-    const bool f = in && row[p.cls[j]] > p.thr;
-    const unsigned int b = __ballot_sync(0xffffffffu, f);
-    if (lane == 0) s_w[warp][j] = __popc(b);
-    if (f) mine |= 1u << j;
-  }
-  __syncthreads();
+  __shared__ uint32_t s_sel[GE_TILES][32];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int t = blockIdx.x * GE_TILES + warp;
+  const int pt = t * 32 + lane;
   int bt = 0;
   float cx = 0.f, cy = 0.f, cz = 0.f;
-  if (mine) {
+  if (pt < p.N) {
     bt = p.batch[pt];
     cx = p.coords[3 * (size_t)pt] + p.offsets[3 * (size_t)pt];
     cy = p.coords[3 * (size_t)pt + 1] + p.offsets[3 * (size_t)pt + 1];
     cz = p.coords[3 * (size_t)pt + 2] + p.offsets[3 * (size_t)pt + 2];
   }
-  for (int j = 0; j < p.nc; j++) {  // every lane stays in the loop: the ballots are full-warp
-    const bool f = (mine >> j) & 1u;
-    const unsigned int b = __ballot_sync(0xffffffffu, f);
-    const int base = p.blk_cnt[(size_t)j * p.nblk + blockIdx.x];
-    // one atomic per (warp, batch item) on the segment counter instead of one per entry (131k adds on <= nc*B words
-    // serialised in L2)
-    const unsigned int peers = __match_any_sync(0xffffffffu, f ? bt : (0x40000000 | lane));
-    if (f && base >= 0 && lane == __ffs(peers) - 1) atomicAdd(&p.seg_cnt[j * p.B + bt], __popc(peers));
-    if (f && base >= 0) {  // base < 0: class dropped by min_npoint
-      int before = 0;
-      for (int w = 0; w < warp; w++) before += s_w[w][j];
-      const int pos = base + before + __popc(b & ((1u << lane) - 1u));
-      p.pts[pos] = pt;
-      const int sg = j * p.B + bt;
-      p.seg[pos] = sg;
-      p.shifted[3 * (size_t)pos] = cx;
-      p.shifted[3 * (size_t)pos + 1] = cy;
-      p.shifted[3 * (size_t)pos + 2] = cz;
+  // lanes of the same batch item: one atomic per (warp, class, batch item) on the segment counter instead of one per entry
+  // (lanes past N never have a selection bit, so their group does not matter)
+  const unsigned int peers = __match_any_sync(0xffffffffu, bt);
+  const unsigned int below = (1u << lane) - 1u;
+  int run = 0;  // entries of the classes before k0
+  for (int k0 = 0; k0 < p.nc; k0 += 32) {
+    const int j = k0 + lane;
+    const int kept = j < p.nc ? p.total[1 + j] : 0;  // 0 for a class dropped by min_npoint: it gets no entries
+    const int incl = warp_incl_scan(kept);
+    const uint32_t m = kept ? p.sel[(size_t)t * p.nc + j] : 0u;
+    __syncthreads();  // the previous chunk's readers of s_sel are done
+    s_sel[warp][lane] = m;
+    __syncthreads();
+    int before = 0;
+    for (int w = 0; w < warp; w++) before += __popc(s_sel[w][lane]);
+    const int base = kept ? run + incl - kept + p.blk_cnt[(size_t)blockIdx.x * p.nc + j] + before : 0;
+    run += __shfl_sync(0xffffffffu, incl, 31);
+    // only the classes this tile has points of (most words are 0 when there are many classes); every lane stays in the
+    // loop: mj and bj are broadcasts
+    for (unsigned int nz = __ballot_sync(0xffffffffu, m != 0u); nz; nz &= nz - 1u) {
+      const int jj = __ffs(nz) - 1;
+      const uint32_t mj = __shfl_sync(0xffffffffu, m, jj);
+      const int bj = __shfl_sync(0xffffffffu, base, jj);
+      if ((mj >> lane) & 1u) {
+        const int pos = bj + __popc(mj & below);
+        const int sg = (k0 + jj) * p.B + bt;
+        p.pts[pos] = pt;
+        p.seg[pos] = sg;
+        p.shifted[3 * (size_t)pos] = cx;
+        p.shifted[3 * (size_t)pos + 1] = cy;
+        p.shifted[3 * (size_t)pos + 2] = cz;
+        const unsigned int g = peers & mj;
+        if (lane == __ffs(g) - 1) atomicAdd(&p.seg_cnt[sg], __popc(g));
+      }
     }
   }
+  if (blockIdx.x == 0 && threadIdx.x == 0) p.total[0] = run;
 }
 
-__global__ void ge_segoff_kernel(GeArgs p) {  // one warp-sized problem: exclusive scan of the (class, batch) counts
-  if (threadIdx.x == 0) {
-    int run = 0;
-    const int n = p.nc * p.B;
-    for (int i = 0; i < n; i++) {
-      p.seg_offsets[i] = run;
-      run += p.seg_cnt[i];
-    }
-    p.seg_offsets[n] = run;
+__global__ void ge_segoff_kernel(GeArgs p) {  // one CTA: exclusive scan of the (class, batch item) counts
+  __shared__ int s_part[32];
+  const int n = p.nc * p.B;
+  int run = 0;
+  for (int i0 = 0; i0 < n; i0 += blockDim.x) {
+    const int i = i0 + threadIdx.x;
+    const int v = i < n ? p.seg_cnt[i] : 0;
+    int sum;
+    const int e = block_excl_scan(v, s_part, sum);
+    if (i < n) p.seg_offsets[i] = run + e;
+    run += sum;
   }
+  if (threadIdx.x == 0) p.seg_offsets[n] = run;
 }
 
 }  // namespace sgb
@@ -171,14 +208,17 @@ extern "C" {
 
 size_t sgb_group_entries_workspace_bytes(int N, int nc, int B) {
   const size_t nblk = (size_t)div_up(std::max(N, 1), GE_THREADS);
-  return align_up((size_t)nc * nblk * 4) + align_up((size_t)nc * (size_t)std::max(B, 1) * 4) + 256;
+  const size_t c = (size_t)std::max(nc, 1);
+  return align_up(nblk * GE_TILES * c * 4) + align_up(nblk * c * 4) + align_up(c * (size_t)std::max(B, 1) * 4) + 256;
 }
 
 int sgb_group_entries(const float *d_scores, int N, int C, const int *h_classes, int nc, float score_thr, int min_npoint,
                       const int32_t *d_batch_idxs, int B, const float *d_coords, const float *d_offsets, int32_t *d_pts,
                       int32_t *d_seg, float *d_shifted, int32_t *d_seg_offsets, int32_t *d_total, void *d_ws, size_t ws_bytes,
                       void *stream) {
-  SGB_REQUIRE(N >= 0 && C >= 1 && nc >= 1 && nc <= GE_MAXC && B >= 1 && h_classes, SGB_ERR_ARG, "group_entries arguments (<= 32 classes per call)");
+  SGB_REQUIRE(N >= 0 && C >= 1 && nc >= 1 && B >= 1 && h_classes, SGB_ERR_ARG, "group_entries arguments");
+  SGB_REQUIRE((long long)N * nc < (1ll << 31) && (long long)nc * B < (1ll << 31), SGB_ERR_RANGE,
+              "group_entries: N * nc entries and nc * B segments must stay below 2^31 (int32 positions)");
   SGB_REQUIRE(d_seg_offsets && d_total && d_ws, SGB_ERR_ARG, "group_entries outputs");
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) {
@@ -188,27 +228,32 @@ int sgb_group_entries(const float *d_scores, int N, int C, const int *h_classes,
   }
   SGB_REQUIRE(d_scores && d_batch_idxs && d_coords && d_offsets && d_pts && d_seg && d_shifted, SGB_ERR_ARG, "group_entries inputs");
   SGB_REQUIRE(ws_bytes >= sgb_group_entries_workspace_bytes(N, nc, B), SGB_ERR_WORKSPACE, "group_entries workspace too small");
+  for (int j = 0; j < nc; j++)
+    SGB_REQUIRE(h_classes[j] >= 0 && h_classes[j] < C, SGB_ERR_RANGE, "group_entries: class id outside the score columns");
   GeArgs p;
   p.scores = d_scores; p.N = N; p.C = C;
-  for (int j = 0; j < nc; j++) {
-    SGB_REQUIRE(h_classes[j] >= 0 && h_classes[j] < C, SGB_ERR_RANGE, "group_entries: class id outside the score columns");
-    p.cls[j] = h_classes[j];
-  }
   p.nc = nc; p.thr = score_thr; p.min_npoint = min_npoint;
   p.batch = d_batch_idxs; p.B = B; p.coords = d_coords; p.offsets = d_offsets;
   p.pts = d_pts; p.seg = d_seg; p.shifted = d_shifted; p.seg_offsets = d_seg_offsets; p.total = d_total;
   p.nblk = div_up(N, GE_THREADS);
   Arena a(d_ws, ws_bytes);
-  p.blk_cnt = a.take<int32_t>((size_t)nc * p.nblk);
+  p.sel = a.take<uint32_t>((size_t)p.nblk * GE_TILES * nc);
+  p.blk_cnt = a.take<int32_t>((size_t)p.nblk * nc);
   p.seg_cnt = a.take<int32_t>((size_t)nc * B);
-  SGB_REQUIRE(p.blk_cnt && p.seg_cnt, SGB_ERR_WORKSPACE, "group_entries workspace carve");
-  ge_count_kernel<<<p.nblk, GE_THREADS, 0, st>>>(p);
-  SGB_LAUNCH_CHECK();
-  ge_scan_kernel<<<1, 1024, 0, st>>>(p);
+  SGB_REQUIRE(p.sel && p.blk_cnt && p.seg_cnt, SGB_ERR_WORKSPACE, "group_entries workspace carve");
+  for (int j0 = 0; j0 < nc; j0 += GE_SLICE) {
+    GeSlice s;
+    s.j0 = j0;
+    s.n = std::min(GE_SLICE, nc - j0);
+    for (int r = 0; r < s.n; r++) s.col[r] = h_classes[j0 + r];
+    ge_count_kernel<<<p.nblk, GE_THREADS, 0, st>>>(p, s);
+    SGB_LAUNCH_CHECK();
+  }
+  ge_scan_kernel<<<nc, GE_SCAN_THREADS, 0, st>>>(p);
   SGB_LAUNCH_CHECK();
   ge_fill_kernel<<<p.nblk, GE_THREADS, 0, st>>>(p);
   SGB_LAUNCH_CHECK();
-  ge_segoff_kernel<<<1, 32, 0, st>>>(p);
+  ge_segoff_kernel<<<1, GE_SCAN_THREADS, 0, st>>>(p);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

@@ -22,8 +22,8 @@ import torch
 import torch.nn as nn
 
 from .. import spconv
-from ..ops import (ball_query, ballquery_batch_p_nosync, bfs_cluster_segments, gather_rows, global_avg_pool, group_entries, sec_max,
-                   sec_min,
+from ..ops import (BALLQUERY_MAX_SEGMENTS, ball_query, ballquery_batch_p_nosync, bfs_cluster_segments, gather_rows, global_avg_pool,
+                   group_entries, sec_max, sec_min,
                    voxelization,
                    voxelization_idx)
 from ..ops import instances as inst_ops
@@ -203,6 +203,8 @@ class SoftGroup(nn.Module):
         tc = self.test_cfg
         eval_tasks = self._cfg(tc, 'eval_tasks', ['semantic', 'instance'])
         x4_split = self._cfg(tc, 'x4_split', False)
+        if not self.semantic_only and ('instance' in eval_tasks or 'panoptic' in eval_tasks):
+            self._grouped_classes(int(batch_size))  # a batch the grouping cannot take fails before the backbone runs
         color_feats = feats
         if self.with_coords:
             feats = torch.cat((feats, coords_float), 1)
@@ -415,6 +417,20 @@ class SoftGroup(nn.Module):
         return x_new
 
     # ------------------------------------------------------------------------------------------------------
+    def _grouped_classes(self, batch_size):
+        """The classes forward_grouping groups. The one-pass grouping hands every (class, batch item) pair to one ball query
+        as a segment; a batch with more segments than it takes raises here, before any launch of the forward."""
+        g = self.grouping_cfg
+        ignore = set(self._cfg(g, 'ignore_classes', []))
+        classes = [c for c in range(self.semantic_classes) if c not in ignore]
+        one_pass = not (self._cfg(g, 'with_pyramid', False) or self._cfg(g, 'with_octree', False))
+        if one_pass and len(classes) * batch_size > BALLQUERY_MAX_SEGMENTS:
+            raise ValueError('forward_grouping: %d grouped classes x batch size %d = %d ball-query segments, more than the %d '
+                             'one ball query takes; run at most %d scans per batch with this config' %
+                             (len(classes), batch_size, len(classes) * batch_size, BALLQUERY_MAX_SEGMENTS,
+                              BALLQUERY_MAX_SEGMENTS // len(classes)))
+        return classes
+
     @force_fp32(apply_to=('semantic_scores, pt_offsets'))
     def forward_grouping(self, semantic_scores, pt_offsets, batch_idxs, coords_float, grouping_cfg=None,
                          lvl_fusion=False, batch_size=None):
@@ -424,18 +440,18 @@ class SoftGroup(nn.Module):
         dev = semantic_scores.device
         if batch_size is None:  # softgroup.py:415 reads it back from the device; forward_test knows it from the collated batch
             batch_size = int(batch_idxs.max().item()) + 1
+        with_pp = self._cfg(g, 'with_pyramid', False) or self._cfg(g, 'with_octree', False)
+        classes = self._grouped_classes(batch_size)
         scores = semantic_scores.softmax(dim=-1)
         radius = float(self._cfg(g, 'radius'))
         mean_active = int(self._cfg(g, 'mean_active'))
         npoint_thr = float(self._cfg(g, 'npoint_thr'))
         score_thr = float(self._cfg(g, 'score_thr'))
-        if self._cfg(g, 'with_pyramid', False) or self._cfg(g, 'with_octree', False):
+        if with_pp:
             return self._forward_grouping_pp(scores, pt_offsets, batch_idxs, coords_float, batch_size,
                                              lvl_fusion=lvl_fusion)
         cnm = self._cfg(g, 'class_numpoint_mean')
         assert len(cnm) == self.semantic_classes
-        ignore = set(self._cfg(g, 'ignore_classes', []))
-        classes = [c for c in range(self.semantic_classes) if c not in ignore]
         min_npoint = int(self._cfg(self.test_cfg, 'min_npoint', 0))
         empty = (torch.zeros((0, 2), dtype=torch.int32, device=dev), torch.zeros((0, ), dtype=torch.int32, device=dev))
         if not classes:

@@ -133,6 +133,9 @@ class BallQueryBatchP(Function):
 
 ballquery_batch_p = BallQueryBatchP.apply
 
+# most segments (batch_offsets.numel() - 1) one ballquery_batch_p call takes (csrc/ballquery.cu kMaxSeg)
+BALLQUERY_MAX_SEGMENTS = 1023
+
 
 def ballquery_batch_p_nosync(coords, batch_idxs, batch_offsets, radius):
     """Device-resident variant for the fused forward: the index buffer is sized for the cap (n * 1000 entries, only
@@ -181,7 +184,7 @@ def gather_rows(feats, idx):
 
 def group_entries(scores, classes, score_thr, min_npoint, batch_idxs, batch_size, coords_float, pt_offsets):
     """All classes of the grouping loop (softgroup/model/softgroup.py:430-446) in one pass on the device: entries in
-    class-major, ascending point order. scores: softmax scores [N, C]; classes: list of class ids (<= 32).
+    class-major, ascending point order. scores: softmax scores [N, C]; classes: list of class ids (any number).
     Returns (pts int32 [cap], seg int32 [cap], shifted float32 [cap, 3], seg_offsets int32 [nc*B+1], total int32 [1+nc]) with
     cap = N * len(classes); only the first total[0] entries are meaningful. No host synchronisation."""
     L = _lib.lib()

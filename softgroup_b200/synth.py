@@ -20,6 +20,10 @@ SHAPES = {
     'c4_kitti': dict(n=120000, room=(60.0, 60.0, 3.0), n_obj=30, sem=19, stuff=tuple(range(0, 11)), scale=20,
                      walls=False),
     'c5_stpls3d': dict(n=1500000, room=(250.0, 250.0, 30.0), n_obj=400, sem=15, stuff=(0, ), scale=3, walls=False),
+    # ScanNet200-shape: a larger room with one object of every one of the 198 grouped classes (spread: object k has thing
+    # class k instead of a random one)
+    'c6_scannet200': dict(n=150000, room=(16.0, 14.0, 3.0), n_obj=198, sem=200, stuff=(0, 1), scale=50, walls=True,
+                          spread=True),
 }
 
 
@@ -69,7 +73,7 @@ def make_scan(shape='c2_scannet', seed=0, n_points=None, batch_id=0):
         size = rng.uniform(smin, smax, 3)
         size[2] = min(size[2], 0.9 * rz)
         lo = np.array([rng.uniform(0, rx - size[0]), rng.uniform(0, ry - size[1]), 0.0])
-        cls = thing_classes[rng.randint(len(thing_classes))]
+        cls = thing_classes[k % len(thing_classes)] if cfg.get('spread') else thing_classes[rng.randint(len(thing_classes))]
         for (o, eu, ev) in _box_faces(lo, lo + size):
             surfaces.append((o, eu, ev, cls, k))
 
