@@ -13,6 +13,15 @@
 //                    the global cursor like the reference (:52), then a coalesced write of the hits -- the
 //                    "first 1000 by index" cap (:43-48) is a loop exit. Stencils larger than the staging area
 //                    fall back to an exact index-order scan of the whole segment.
+// Routing of a work item (total_s = points in the stencil, nwords = its id range in 32-bit words):
+//    pass 0, bitmap    total_s <= 5120    nwords <= 4096
+//    pass 0, bitonic   total_s <= 4096    nwords >  4096
+//    pass 1, bitmap    total_s <= 10240   nwords <= 8192   (items pass 0 did not take)
+//    pass 1, bitonic   total_s <= 8192    nwords >  8192
+//    exact scan        everything else
+// The bitonic sort pads the stencil to P = pow2 >= total_s records, so it runs only where P fits the staging area
+// (total_s <= kSortMax); a wider stencil goes on to the next configuration. tests/neighbour_cases.py restates this
+// routing on the CPU.
 // Exactness: the distance is evaluated with the reference's compiled contraction order
 //   d2 = fma(dz,dz, fma(dx,dx, dy*dy)),  hit iff d2 < radius*radius   (strict, fp32)
 // and any pair with d2 < r^2 differs by < h in every coordinate, so it lies in the 27-cell stencil.
@@ -33,8 +42,14 @@ namespace sgb {
 // configuration alone is faster on fragmented predictions but slower on the clean 40-object scan, whose cores overflow
 // into the exact-scan path.
 template <int PASS> struct BqCfg;
-template <> struct BqCfg<0> { static constexpr int kThreads = 512, kSMax = 5120, kBmWords = 4096, kPerSM = 2; };
-template <> struct BqCfg<1> { static constexpr int kThreads = 1024, kSMax = 10240, kBmWords = 8192, kPerSM = 1; };
+// kSortMax: the largest power of two <= kSMax, the most records the bitonic fallback can pad and sort in S[].
+template <> struct BqCfg<0> { static constexpr int kThreads = 512, kSMax = 5120, kSortMax = 4096, kBmWords = 4096, kPerSM = 2; };
+template <> struct BqCfg<1> { static constexpr int kThreads = 1024, kSMax = 10240, kSortMax = 8192, kBmWords = 8192, kPerSM = 1; };
+template <int PASS> constexpr bool bq_sort_max_ok() {
+  constexpr int m = BqCfg<PASS>::kSortMax, s = BqCfg<PASS>::kSMax;
+  return (m & (m - 1)) == 0 && m <= s && 2 * m > s;
+}
+static_assert(bq_sort_max_ok<0>() && bq_sort_max_ok<1>(), "kSortMax must be the largest power of two <= kSMax");
 constexpr int kCellBias = 131072;
 constexpr int kMaxSeg = 1023;
 
@@ -245,19 +260,22 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
     const int total_s = nb_off[27];
     const int q_first = w.chunk_q0[item];
     const int q_start = w.slot_start[cslot] + q_first, q_cnt = min(kBqChunk, w.slot_cnt[cslot] - q_first);
-    if (PASS == 0 && total_s > kBqSMax) {  // too large for this configuration's staging area: left to pass 1
+    const int lo = s_lo;
+    const int nwords = (s_hi - lo + 32) >> 5;
+    const bool use_bitmap = nwords <= kBmWords;
+    // the bitonic fallback pads the stencil to a power of two >= total_s, which has to fit S[] too
+    const bool staged = total_s <= (use_bitmap ? kBqSMax : BqCfg<PASS>::kSortMax);
+    if (PASS == 0 && !staged) {  // too large for this configuration's staging area: left to pass 1
       if (tid == 0) w.big_items[atomicAdd(&w.scalars[5], 1)] = item;
       continue;
     }
 
-    if (total_s <= kBqSMax) {
+    if (staged) {
       // ---- order the stencil by point index. Point indices are distinct, so the sorted position of a record is
       //      the number of stencil members with a smaller index: one bit per index in a shared-memory bitmap +
       //      prefix popcounts gives it in O(|S| + range/32) instead of an O(|S| log^2 |S|) bitonic sort.
-      const int lo = s_lo;
-      const int nwords = (s_hi - lo + 32) >> 5;
       bool ordered = false;
-      if (nwords <= kBmWords) {
+      if (use_bitmap) {
         for (int t = tid; t < nwords; t += kBqThreads) bm[t] = 0u;
         __syncthreads();
         for (int k = 0; k < 27; k++) {
@@ -302,7 +320,7 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
         ordered = true;
       }
       if (!ordered) {
-      // ---- index range too wide for the bitmap: stage the stencil and bitonic-sort it ---------------------
+      // ---- index range too wide for the bitmap: stage the stencil and bitonic-sort it (P <= kSortMax) ----
       int P = 32;
       while (P < total_s) P <<= 1;
       for (int k = 0; k < 27; k++) {
@@ -398,7 +416,7 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
         __syncwarp();
       }
     } else {
-      // ---- oversize stencil (> kBqSMax candidates): exact index-order scan of the segment ---------
+      // ---- stencil beyond pass 1's staging area: exact index-order scan of the segment ---------------
       for (int q = warp; q < q_cnt; q += kBqWarps) {
         float4 qp = w.sorted[q_start + q];
         int qi = __float_as_int(qp.w);
@@ -471,7 +489,7 @@ static int bq_launch(int n, long long capacity, float radius, const float *xyz, 
   bq_query_kernel<0><<<std::min(std::max(n, 1), BqCfg<0>::kPerSM * kNumSMs), BqCfg<0>::kThreads, smem0, st>>>(
       xyz, batch_idxs, batch_offsets, n, radius, capacity, idx, start_len, w);
   SGB_LAUNCH_CHECK();
-  // the items pass 0 noted (stencils of 5121..10240 candidates stay on the staged path; beyond that the exact scan)
+  // the items pass 0 noted (stencils of up to 10240 candidates stay on the staged path; beyond that the exact scan)
   bq_query_kernel<1><<<std::min(std::max(n, 1), kNumSMs), BqCfg<1>::kThreads, smem1, st>>>(xyz, batch_idxs, batch_offsets, n, radius,
                                                                                          capacity, idx, start_len, w);
   SGB_LAUNCH_CHECK();

@@ -122,7 +122,8 @@ def test_ballquery_vs_oracle(n, B, r, sigma):
 
 
 def test_ballquery_cap_and_oversize_cell():
-    # > 4096 candidates in one stencil (brute-force path) and > 1000 neighbours (cap = first 1000 by index)
+    # 5000 candidates in one stencil (pass 0's staged path, just under its 5120 records; the exact scan and the other
+    # paths are in test_gpu_neighbour_edges.py) and > 1000 neighbours (cap = first 1000 by index)
     rng = np.random.RandomState(1)
     xyz = (rng.randn(6000, 3) * 0.004).astype(np.float32)
     xyz[5000:] += 1.0
