@@ -86,11 +86,12 @@ int sgb_voxelize_bp(const float *d_d_out, float *d_d_feats, const int32_t *d_rul
  * exactly like the reference (:55-61) and the caller relaunches with a larger meanActive
  * (softgroup/ops/functions.py:258-266). d_start_len int32 [n,2] = (start, count).
  * Returns (blocking) the total neighbour count, like the reference's `return cumsum`.
- * The *_async form never synchronises: it leaves d_total[0] = total, d_total[1] = range-error flag (int32 [2], device).
+ * The *_async form never synchronises: it leaves d_total[0] = total, d_total[1] = error flags (int32 [2], device).
  * Points with a NaN / Inf coordinate get the empty list and are nobody's neighbour -- the reference's result, every
  * comparison with them being false (:38-44). B must be <= 1023 and finite |xyz/radius| < 131070: SGB_ERR_RANGE
- * otherwise (blocking form), or the flag in d_total[1] (async form; sgb_bfs_cluster_count reports it).
- * capacity must stay below 2^31 entries (int32 cursor).
+ * otherwise (blocking form), or bit 1 of d_total[1] (async form; sgb_bfs_cluster_count reports it).
+ * capacity must stay below 2^31 entries (int32 cursor). A neighbour total beyond 2^31 - 1 does not fit the int32 cursor
+ * either: nothing is written past the wrap, and it is SGB_ERR_RANGE (blocking form) or bit 2 of d_total[1].
  * ------------------------------------------------------------------------------------------- */
 size_t sgb_ballquery_workspace_bytes(int n);
 long long sgb_ballquery_batch_p(int n, int meanActive, float radius, const float *d_xyz, const int32_t *d_batch_idxs,
@@ -128,7 +129,7 @@ long long sgb_octree_ball_query(const float *d_points, const float *d_boxes, con
  * The labelling is the exact directed one (lists cut by the 1000 cap make the graph asymmetric); label passes are
  * enqueued in batches and the host waits ONCE, for the totals. d_upstream_err (nullable): device int32 error flag of
  * the asynchronous ball query that produced the lists (d_total + 1 of sgb_ballquery_batch_p_async); it is read at that
- * same wait and reported as SGB_ERR_RANGE.
+ * same wait and reported as SGB_ERR_RANGE when non-zero.
  * ------------------------------------------------------------------------------------------- */
 size_t sgb_bfs_cluster_workspace_bytes(int N);
 int sgb_bfs_cluster_count(const int32_t *d_ball_query_idxs, const int32_t *d_start_len, int N, float thr,

@@ -183,6 +183,14 @@ __device__ __forceinline__ bool bq_hit(float qx, float qy, float qz, float x, fl
   return d2 < r2;
 }
 
+// The list cursor w.scalars[3] is int32 like the reference's. A neighbour total beyond 2^31 - 1 wraps it: the list that
+// crosses 2^31 - 1 raises bit 2 of the error flag, and every later (negative) base writes nothing -- the lists are then
+// incomplete, and the flag makes the caller's next synchronisation fail instead of clustering them. Below the limit
+// nothing changes: a base is never negative and the crossing never happens.
+__device__ __forceinline__ void bq_check_cursor(int base, int cnt, const BqWs &w) {
+  if (base < 0 || (long long)base + cnt > 0x7fffffffll) atomicOr(&w.scalars[2], 2);
+}
+
 // Emit one query's list: staged hits (ascending) -> global, reference truncation rules (bfs_cluster.cu:52-65).
 __device__ __forceinline__ void bq_emit(int qi, int cnt, const int32_t *stage, int32_t *__restrict__ idx,
                                         int32_t *__restrict__ start_len, int32_t *total, long long capacity, int lane) {
@@ -396,8 +404,9 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
           start_len[2 * (size_t)qi + 1] = cnt;
         }
         base = __shfl_sync(0xffffffffu, base, 0);
+        if (lane == 0) bq_check_cursor(base, cnt, w);
         const long long room = capacity - (long long)base;  // reference truncation (bfs_cluster.cu:55-61)
-        const int cw = (room <= 0) ? 0 : (((long long)base + cnt >= capacity) ? (int)room : cnt);
+        const int cw = (base < 0 || room <= 0) ? 0 : (((long long)base + cnt >= capacity) ? (int)room : cnt);
         int32_t *__restrict__ out = idx + base;
         int done = 0;
         uint32_t wa = s_addr + (uint32_t)lane * 16u + 12u;  // the index word of this lane's candidate
@@ -437,8 +446,9 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
           start_len[2 * (size_t)qi + 1] = cnt;
         }
         base = __shfl_sync(0xffffffffu, base, 0);
+        if (lane == 0) bq_check_cursor(base, cnt, w);
         long long room = capacity - (long long)base;
-        int cw = (room <= 0) ? 0 : (((long long)base + cnt >= capacity) ? (int)room : cnt);
+        int cw = (base < 0 || room <= 0) ? 0 : (((long long)base + cnt >= capacity) ? (int)room : cnt);
         int done = 0;
         for (int b0 = s0; b0 < last && done < cw; b0 += 32) {
           int t = b0 + lane;
@@ -547,7 +557,8 @@ long long sgb_ballquery_batch_p(int n, int meanActive, float radius, const float
   int h[4];
   SGB_CUDA_CHECK(cudaMemcpyAsync(h, w.scalars, sizeof(h), cudaMemcpyDeviceToHost, st));
   SGB_CUDA_CHECK(cudaStreamSynchronize(st));
-  SGB_REQUIRE(h[2] == 0, SGB_ERR_RANGE, "ballquery: |xyz/radius| >= 131070 or batch index outside [0,1023]");
+  SGB_REQUIRE((h[2] & 1) == 0, SGB_ERR_RANGE, "ballquery: |xyz/radius| >= 131070 or batch index outside [0,1023]");
+  SGB_REQUIRE(h[2] == 0, SGB_ERR_RANGE, "ballquery: neighbour total beyond 2^31 - 1 (int32 list cursor)");
   return (long long)h[3];
 }
 }

@@ -540,7 +540,8 @@ int sgb_bfs_cluster_count(const int32_t *d_ball_query_idxs, const int32_t *d_sta
     SGB_CUDA_CHECK(cudaMemcpyAsync(sc, w.scalars, sizeof(sc), cudaMemcpyDeviceToHost, st));
     if (d_upstream_err && batch == 0) SGB_CUDA_CHECK(cudaMemcpyAsync(&up_err, d_upstream_err, 4, cudaMemcpyDeviceToHost, st));
     SGB_CUDA_CHECK(cudaStreamSynchronize(st));
-    SGB_REQUIRE(up_err == 0, SGB_ERR_RANGE, "ball query upstream of bfs_cluster: |xyz/radius| >= 131070 or segment id outside [0,1023]");
+    SGB_REQUIRE((up_err & 1) == 0, SGB_ERR_RANGE, "ball query upstream of bfs_cluster: |xyz/radius| >= 131070 or segment id outside [0,1023]");
+    SGB_REQUIRE(up_err == 0, SGB_ERR_RANGE, "ball query upstream of bfs_cluster: neighbour total beyond 2^31 - 1 (int32 list cursor)");
     if (sc[8 + kBatch - 1] == 0) break;  // the last pass of the batch pushed nothing: fixed point
   }
   if (h_maxLen) *h_maxLen = sc[1];

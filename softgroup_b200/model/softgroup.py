@@ -26,7 +26,9 @@ from ..ops import (BALLQUERY_MAX_SEGMENTS, ball_query, ballquery_batch_p_nosync,
                    group_entries, sec_max, sec_min,
                    voxelization,
                    voxelization_idx)
+from ..ops import functions
 from ..ops import instances as inst_ops
+from ..ops._lib import SgbError
 from ..util import cuda_cast, force_fp32, rle_encode_ids
 from .blocks import MLP, ResidualBlock, UBlock
 
@@ -465,16 +467,11 @@ class SoftGroup(nn.Module):
         if n == 0:
             return empty
         pts, seg, shifted = pts[:n], seg[:n], shifted[:n]
+        if n * 1000 > functions.BALLQUERY_MAX_CAPACITY:
+            seg_thr = self._seg_thr(classes, batch_size, npoint_thr, cnm, dev)
+            return self._group_chunks(pts, seg, shifted, seg_offsets, seg_thr, radius, empty)
         neighbor_inds, start_len, n_active = ballquery_batch_p_nosync(shifted, seg, seg_offsets, radius)
-        # per-segment thresholds: threshold*mean or absolute when mean == -1 (bfs_cluster.cpp:70-77), float32 math
-        key = (tuple(classes), batch_size, npoint_thr, str(dev))
-        hit = self.__dict__.get('_seg_thr_cache')
-        if hit is None or hit[0] != key:
-            thr_c = [npoint_thr if cnm[c] == -1 else float(np.float32(npoint_thr) * np.float32(cnm[c])) for c in classes]
-            seg_thr = torch.tensor(np.repeat(np.asarray(thr_c, np.float32), batch_size), dtype=torch.float32, device=dev)
-            hit = (key, seg_thr)
-            self.__dict__['_seg_thr_cache'] = hit
-        seg_thr = hit[1]
+        seg_thr = self._seg_thr(classes, batch_size, npoint_thr, cnm, dev)
         # lists that hit the 1000 cap make the graph asymmetric: the labelling is the exact directed one
         cidx, coff = bfs_cluster_segments(neighbor_inds, start_len, 0.0, node_seg=seg, seg_thr=seg_thr,
                                           nactive=n_active[0:1], upstream_err=n_active[1:2])
@@ -483,6 +480,56 @@ class SoftGroup(nn.Module):
         # proposals_idx[:, 1] = object_idxs[proposals_idx[:, 1]] (:464)
         cidx[:, 1] = pts[cidx[:, 1].long()].int()
         return cidx, coff
+
+    def _seg_thr(self, classes, batch_size, npoint_thr, cnm, dev):
+        """Per-segment thresholds: threshold*mean or absolute when mean == -1 (bfs_cluster.cpp:70-77), float32 math."""
+        key = (tuple(classes), batch_size, npoint_thr, str(dev))
+        hit = self.__dict__.get('_seg_thr_cache')
+        if hit is None or hit[0] != key:
+            thr_c = [npoint_thr if cnm[c] == -1 else float(np.float32(npoint_thr) * np.float32(cnm[c])) for c in classes]
+            seg_thr = torch.tensor(np.repeat(np.asarray(thr_c, np.float32), batch_size), dtype=torch.float32, device=dev)
+            hit = (key, seg_thr)
+            self.__dict__['_seg_thr_cache'] = hit
+        return hit[1]
+
+    def _group_chunks(self, pts, seg, shifted, seg_offsets, seg_thr, radius, empty):
+        """forward_grouping for a selection whose worst-case neighbour buffer (1000 per entry) is beyond the ball query's
+        int32 cursor: the segments are cut into chunks that fit (functions.plan_ballquery_chunks), each chunk runs the
+        same ball query and clustering, and the results are concatenated in chunk order. A neighbour list never leaves
+        its segment, so no component crosses a chunk, and the clustering numbers components in node order: the
+        concatenation is what one call without the limit returns. A segment that alone is beyond the limit runs with
+        the largest buffer; when its real neighbour total does not fit either, SgbError is raised before clustering."""
+        seg_off = seg_offsets.cpu().numpy().astype(np.int64)  # the second host read, only above the limit
+        idx_list, off_list = [], []
+        n_prop, n_pts = 0, 0
+        for s0, s1 in functions.plan_ballquery_chunks(np.diff(seg_off)):
+            e0, e1 = int(seg_off[s0]), int(seg_off[s1])
+            m = e1 - e0
+            if m == 0:
+                continue
+            c_seg = seg[e0:e1] - s0
+            c_off = seg_offsets[s0:s1 + 1] - e0
+            capacity = min(m * 1000, functions.BALLQUERY_MAX_CAPACITY)
+            neighbor_inds, start_len, n_active = ballquery_batch_p_nosync(shifted[e0:e1], c_seg, c_off, radius,
+                                                                          capacity=capacity)
+            if m * 1000 > capacity:  # one oversize segment: its lists may not have fit
+                t, flags = (int(v) for v in n_active.cpu())
+                if flags & functions.BALLQUERY_ERR_CURSOR or t > capacity:
+                    raise SgbError('forward_grouping: segment %d (%d entries) has more neighbours than one ball query '
+                                   'holds (%d; its int32 list cursor addresses at most 2^31 - 1)' % (s0, m, capacity))
+            cidx, coff = bfs_cluster_segments(neighbor_inds, start_len, 0.0, node_seg=c_seg, seg_thr=seg_thr[s0:s1],
+                                              nactive=n_active[0:1], upstream_err=n_active[1:2])
+            if cidx.size(0) == 0:
+                continue
+            cidx[:, 1] = pts[e0:e1][cidx[:, 1].long()].int()
+            cidx[:, 0] += n_prop
+            idx_list.append(cidx)
+            off_list.append(coff[1:] + n_pts if off_list else coff)
+            n_prop += coff.numel() - 1
+            n_pts += cidx.size(0)
+        if not idx_list:
+            return empty
+        return torch.cat(idx_list, 0), torch.cat(off_list)
 
     # ------------------------------------------------------------------------------------------------------
     def _forward_grouping_pp(self, scores, pt_offsets, batch_idxs, coords_float, batch_size, lvl_fusion=False):

@@ -135,15 +135,48 @@ ballquery_batch_p = BallQueryBatchP.apply
 
 # most segments (batch_offsets.numel() - 1) one ballquery_batch_p call takes (csrc/ballquery.cu kMaxSeg)
 BALLQUERY_MAX_SEGMENTS = 1023
+# largest neighbour-index buffer one ball query addresses: its list cursor and start_len are int32
+BALLQUERY_MAX_CAPACITY = 2**31 - 1
+# flag bit in total[1] of ballquery_batch_p_nosync: the neighbour total passed 2^31 - 1 (csrc/ballquery.cu)
+BALLQUERY_ERR_CURSOR = 2
 
 
-def ballquery_batch_p_nosync(coords, batch_idxs, batch_offsets, radius):
+def plan_ballquery_chunks(seg_counts, max_capacity=None):
+    """Cut segments into contiguous ranges [s0, s1) for one ball query each, greedily in segment order, so that every
+    range's worst-case index buffer (1000 entries per point) fits: sum(seg_counts[s0:s1]) * 1000 <= max_capacity
+    (default BALLQUERY_MAX_CAPACITY). A segment that alone exceeds it gets a range of its own. The ranges tile
+    [0, len(seg_counts)); a range may hold no entries (empty segments next to an oversize one)."""
+    if max_capacity is None:
+        max_capacity = BALLQUERY_MAX_CAPACITY
+    limit = max_capacity // 1000  # most entries a chunk takes
+    chunks, s0, acc = [], 0, 0
+    for s, c in enumerate(int(c) for c in seg_counts):
+        if c > limit:  # oversize: close the open range, then a range of its own
+            if s > s0:
+                chunks.append((s0, s))
+            chunks.append((s, s + 1))
+            s0, acc = s + 1, 0
+        elif acc + c > limit:
+            chunks.append((s0, s))
+            s0, acc = s, c
+        else:
+            acc += c
+    if s0 < len(seg_counts):
+        chunks.append((s0, len(seg_counts)))
+    return chunks
+
+
+def ballquery_batch_p_nosync(coords, batch_idxs, batch_offsets, radius, capacity=None):
     """Device-resident variant for the fused forward: the index buffer is sized for the cap (n * 1000 entries, only
     the used prefix is ever touched), so there is no overflow relaunch (functions.py:258-266 of the reference) and
     no host synchronisation. Returns (idx buffer int32 [n*1000], start_len int32 [n,2], total int32 [2] on device:
-    [sum of list lengths, range-error flag]); only idx[start:start+len] per point is meaningful. The error flag is
+    [sum of list lengths, error flags]); only idx[start:start+len] per point is meaningful. The error flags are
     reported by the next bfs_cluster_segments(..., upstream_err=total[1:]) at its own synchronisation. The buffer is
-    4 KB per entry (0.5 GB at 131k entries, 3.2 GB at 800k): sized for 180 GB of HBM, int32 cursor => n < 2^31/1000."""
+    4 KB per entry (0.5 GB at 131k entries, 3.2 GB at 800k); the int32 list cursor limits it to n < 2^31/1000 entries
+    (plan_ballquery_chunks cuts larger selections).
+    capacity: a smaller buffer (at most BALLQUERY_MAX_CAPACITY) for a segment whose n * 1000 exceeds that; lists beyond
+    it are truncated, which total[0] > capacity shows, and a neighbour total beyond 2^31 - 1 sets
+    BALLQUERY_ERR_CURSOR in total[1]. The caller has to check both before clustering."""
     n = coords.size(0)
     assert coords.is_contiguous() and coords.is_cuda
     L = _lib.lib()
@@ -151,8 +184,12 @@ def ballquery_batch_p_nosync(coords, batch_idxs, batch_offsets, radius):
     B = batch_offsets.numel() - 1
     start_len = torch.empty((n, 2), dtype=torch.int32, device=dev)
     total = torch.zeros(2, dtype=torch.int32, device=dev)
-    assert n * 1000 < 2**31, 'ballquery_batch_p_nosync: %d entries need an index buffer beyond the int32 cursor' % n
-    cap = max(n, 1) * 1000
+    if capacity is None:
+        assert n * 1000 < 2**31, 'ballquery_batch_p_nosync: %d entries need an index buffer beyond the int32 cursor' % n
+        cap = max(n, 1) * 1000
+    else:
+        cap = int(capacity)
+        assert 1 <= cap <= BALLQUERY_MAX_CAPACITY, 'ballquery_batch_p_nosync: capacity %d outside [1, 2^31 - 1]' % cap
     idx = torch.empty(cap, dtype=torch.int32, device=dev)
     if n == 0:
         return idx, start_len, total
