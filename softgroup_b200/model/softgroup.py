@@ -9,7 +9,9 @@ What is restructured underneath (same outputs):
     class becomes ONE segmented ball query + ONE clustering call -- class c of batch item b is segment
     (rank(c), b); segments are contiguous because entries are taken class-major in ascending point order,
     which is exactly the order in which the reference concatenates its per-class results. Neighbour lists
-    never leave the GPU (the reference copies them to the CPU for BFS, :458).
+    never leave the GPU (the reference copies them to the CPU for BFS, :458). The call runs once per range of
+    segments: one range holding every segment, or, for a selection beyond the ball query's int32 list cursor,
+    the ranges of plan_ballquery_chunks, concatenated in order.
   * clusters_voxelization (:655-709): the hash runs on the GPU (the reference moves coords to the CPU, :701-703).
   * get_instances (:537-604): no dense [nProposal, N] int masks; per (proposal, class) point counts come from a
     segmented sum, kept masks are encoded to the reference's RLE wire format from sorted point ids.
@@ -50,6 +52,26 @@ def expand_voxel_entries(proposals_idx, v2p_map, num_voxels):
     pts = pts_by_voxel[start[vox[row_of]] + within]
     out = torch.stack([proposals_idx[row_of, 0].long(), pts], 1).int().contiguous()
     return out, row_of
+
+
+def _concat_proposals(parts, device):
+    """Non-empty (cluster_idxs int32 [S, 2], cluster_offsets int32 [nCluster+1]) parts with global point ids -> one
+    (proposals_idx, proposals_offset): cluster ids shifted by the clusters of the parts before, offsets by their
+    entries. One part is returned as it is; no part gives the empty pair int32 [0, 2], [0]."""
+    if len(parts) == 1:
+        return parts[0]
+    if not parts:
+        return (torch.zeros((0, 2), dtype=torch.int32, device=device),
+                torch.zeros((0, ), dtype=torch.int32, device=device))
+    idx_list, off_list = [], []
+    n_prop, n_pts = 0, 0
+    for cidx, coff in parts:
+        cidx[:, 0] += n_prop
+        idx_list.append(cidx)
+        off_list.append(coff[1:] + n_pts if off_list else coff)
+        n_prop += coff.numel() - 1
+        n_pts += cidx.size(0)
+    return torch.cat(idx_list, 0), torch.cat(off_list)
 
 
 class _HostFetcher(object):
@@ -442,22 +464,19 @@ class SoftGroup(nn.Module):
         dev = semantic_scores.device
         if batch_size is None:  # softgroup.py:415 reads it back from the device; forward_test knows it from the collated batch
             batch_size = int(batch_idxs.max().item()) + 1
-        with_pp = self._cfg(g, 'with_pyramid', False) or self._cfg(g, 'with_octree', False)
         classes = self._grouped_classes(batch_size)
         scores = semantic_scores.softmax(dim=-1)
         radius = float(self._cfg(g, 'radius'))
-        mean_active = int(self._cfg(g, 'mean_active'))
         npoint_thr = float(self._cfg(g, 'npoint_thr'))
         score_thr = float(self._cfg(g, 'score_thr'))
-        if with_pp:
-            return self._forward_grouping_pp(scores, pt_offsets, batch_idxs, coords_float, batch_size,
-                                             lvl_fusion=lvl_fusion)
         cnm = self._cfg(g, 'class_numpoint_mean')
-        assert len(cnm) == self.semantic_classes
         min_npoint = int(self._cfg(self.test_cfg, 'min_npoint', 0))
-        empty = (torch.zeros((0, 2), dtype=torch.int32, device=dev), torch.zeros((0, ), dtype=torch.int32, device=dev))
+        if self._cfg(g, 'with_pyramid', False) or self._cfg(g, 'with_octree', False):
+            return self._forward_grouping_pp(scores, pt_offsets, batch_idxs, coords_float, batch_size, classes, radius,
+                                             npoint_thr, score_thr, cnm, min_npoint, lvl_fusion=lvl_fusion)
+        assert len(cnm) == self.semantic_classes
         if not classes:
-            return empty
+            return _concat_proposals([], dev)
         # every class of the loop :430-446 in one pass (csrc/grouping.cu): entries (class rank, point) in class-major,
         # ascending point order, their ball-query segments rank(c) * B + b and shifted coordinates; classes below min_npoint
         # are dropped like `object_idxs.size(0) < min_npoint -> continue` (:437-439)
@@ -465,96 +484,70 @@ class SoftGroup(nn.Module):
                                                               batch_size, coords_float, pt_offsets)
         n = int(total[0].item())  # the one host synchronisation of the selection (the list buffers are sized from it)
         if n == 0:
-            return empty
-        pts, seg, shifted = pts[:n], seg[:n], shifted[:n]
-        if n * 1000 > functions.BALLQUERY_MAX_CAPACITY:
-            seg_thr = self._seg_thr(classes, batch_size, npoint_thr, cnm, dev)
-            return self._group_chunks(pts, seg, shifted, seg_offsets, seg_thr, radius, empty)
-        neighbor_inds, start_len, n_active = ballquery_batch_p_nosync(shifted, seg, seg_offsets, radius)
+            return _concat_proposals([], dev)
         seg_thr = self._seg_thr(classes, batch_size, npoint_thr, cnm, dev)
-        # lists that hit the 1000 cap make the graph asymmetric: the labelling is the exact directed one
-        cidx, coff = bfs_cluster_segments(neighbor_inds, start_len, 0.0, node_seg=seg, seg_thr=seg_thr,
-                                          nactive=n_active[0:1], upstream_err=n_active[1:2])
-        if cidx.size(0) == 0:
-            return empty
-        # proposals_idx[:, 1] = object_idxs[proposals_idx[:, 1]] (:464)
-        cidx[:, 1] = pts[cidx[:, 1].long()].int()
-        return cidx, coff
+        # one ball query and clustering per range (s0, s1) of segments, entries [e0, e1). A selection whose list buffer
+        # (1000 per entry) is beyond the int32 list cursor is cut into ranges that fit, at one more host read. No
+        # neighbour list leaves its segment and components are numbered in node order: the concatenation is one call's.
+        ranges = [(0, len(classes) * batch_size, 0, n)]
+        if n * 1000 > functions.BALLQUERY_MAX_CAPACITY:
+            seg_off = seg_offsets.cpu().numpy().astype(np.int64)
+            ranges = [(s0, s1, int(seg_off[s0]), int(seg_off[s1]))
+                      for s0, s1 in functions.plan_ballquery_chunks(np.diff(seg_off))]
+        parts = []
+        for s0, s1, e0, e1 in ranges:
+            m = e1 - e0
+            if m == 0:
+                continue
+            r_seg, r_off = seg[e0:e1], seg_offsets[s0:s1 + 1]
+            if s0 > 0:  # rebased to the range
+                r_seg, r_off = r_seg - s0, r_off - e0
+            if m * 1000 <= functions.BALLQUERY_MAX_CAPACITY:  # the worst-case buffer fits: m * 1000 entries
+                neighbor_inds, start_len, n_active = ballquery_batch_p_nosync(shifted[e0:e1], r_seg, r_off, radius)
+            else:  # a segment alone beyond the bound: the largest buffer, and SgbError before clustering if it overflows
+                capacity = functions.BALLQUERY_MAX_CAPACITY
+                neighbor_inds, start_len, n_active = ballquery_batch_p_nosync(shifted[e0:e1], r_seg, r_off, radius,
+                                                                              capacity=capacity)
+                t, flags = (int(v) for v in n_active.cpu())
+                if flags & functions.BALLQUERY_ERR_CURSOR or t > capacity:
+                    raise SgbError('forward_grouping: segment %d (%d entries) has more neighbours than one ball query '
+                                   'holds (%d; its int32 list cursor addresses at most 2^31 - 1)' % (s0, m, capacity))
+            # lists that hit the 1000 cap make the graph asymmetric: the labelling is the exact directed one
+            cidx, coff = bfs_cluster_segments(neighbor_inds, start_len, 0.0, node_seg=r_seg, seg_thr=seg_thr[s0:s1],
+                                              nactive=n_active[0:1], upstream_err=n_active[1:2])
+            if cidx.size(0) == 0:
+                continue
+            # proposals_idx[:, 1] = object_idxs[proposals_idx[:, 1]] (:464)
+            cidx[:, 1] = pts[e0:e1][cidx[:, 1].long()].int()
+            parts.append((cidx, coff))
+        return _concat_proposals(parts, dev)
 
     def _seg_thr(self, classes, batch_size, npoint_thr, cnm, dev):
-        """Per-segment thresholds: threshold*mean or absolute when mean == -1 (bfs_cluster.cpp:70-77), float32 math."""
+        """Per-segment thresholds on the device: functions.cluster_threshold of every class, once per batch item."""
         key = (tuple(classes), batch_size, npoint_thr, str(dev))
         hit = self.__dict__.get('_seg_thr_cache')
         if hit is None or hit[0] != key:
-            thr_c = [npoint_thr if cnm[c] == -1 else float(np.float32(npoint_thr) * np.float32(cnm[c])) for c in classes]
+            thr_c = [functions.cluster_threshold(npoint_thr, cnm[c]) for c in classes]
             seg_thr = torch.tensor(np.repeat(np.asarray(thr_c, np.float32), batch_size), dtype=torch.float32, device=dev)
             hit = (key, seg_thr)
             self.__dict__['_seg_thr_cache'] = hit
         return hit[1]
 
-    def _group_chunks(self, pts, seg, shifted, seg_offsets, seg_thr, radius, empty):
-        """forward_grouping for a selection whose worst-case neighbour buffer (1000 per entry) is beyond the ball query's
-        int32 cursor: the segments are cut into chunks that fit (functions.plan_ballquery_chunks), each chunk runs the
-        same ball query and clustering, and the results are concatenated in chunk order. A neighbour list never leaves
-        its segment, so no component crosses a chunk, and the clustering numbers components in node order: the
-        concatenation is what one call without the limit returns. A segment that alone is beyond the limit runs with
-        the largest buffer; when its real neighbour total does not fit either, SgbError is raised before clustering."""
-        seg_off = seg_offsets.cpu().numpy().astype(np.int64)  # the second host read, only above the limit
-        idx_list, off_list = [], []
-        n_prop, n_pts = 0, 0
-        for s0, s1 in functions.plan_ballquery_chunks(np.diff(seg_off)):
-            e0, e1 = int(seg_off[s0]), int(seg_off[s1])
-            m = e1 - e0
-            if m == 0:
-                continue
-            c_seg = seg[e0:e1] - s0
-            c_off = seg_offsets[s0:s1 + 1] - e0
-            capacity = min(m * 1000, functions.BALLQUERY_MAX_CAPACITY)
-            neighbor_inds, start_len, n_active = ballquery_batch_p_nosync(shifted[e0:e1], c_seg, c_off, radius,
-                                                                          capacity=capacity)
-            if m * 1000 > capacity:  # one oversize segment: its lists may not have fit
-                t, flags = (int(v) for v in n_active.cpu())
-                if flags & functions.BALLQUERY_ERR_CURSOR or t > capacity:
-                    raise SgbError('forward_grouping: segment %d (%d entries) has more neighbours than one ball query '
-                                   'holds (%d; its int32 list cursor addresses at most 2^31 - 1)' % (s0, m, capacity))
-            cidx, coff = bfs_cluster_segments(neighbor_inds, start_len, 0.0, node_seg=c_seg, seg_thr=seg_thr[s0:s1],
-                                              nactive=n_active[0:1], upstream_err=n_active[1:2])
-            if cidx.size(0) == 0:
-                continue
-            cidx[:, 1] = pts[e0:e1][cidx[:, 1].long()].int()
-            cidx[:, 0] += n_prop
-            idx_list.append(cidx)
-            off_list.append(coff[1:] + n_pts if off_list else coff)
-            n_prop += coff.numel() - 1
-            n_pts += cidx.size(0)
-        if not idx_list:
-            return empty
-        return torch.cat(idx_list, 0), torch.cat(off_list)
-
     # ------------------------------------------------------------------------------------------------------
-    def _forward_grouping_pp(self, scores, pt_offsets, batch_idxs, coords_float, batch_size, lvl_fusion=False):
+    def _forward_grouping_pp(self, scores, pt_offsets, batch_idxs, coords_float, batch_size, classes, base_radius,
+                             npoint_thr, score_thr, cnm, min_npoint, lvl_fusion=False):
         """SoftGroup++ grouping (softgroup.py:427-463, 482-507): per class, optional pyramid re-voxelisation at
         base_size*level, octree ball query, clustering, inverse pyramid map -- every step on the GPU (the reference
         hashes on the CPU at :494 and builds a dense [nCluster, n] CPU matrix at :500-507). The radius and the level
         depend on the class size, so classes stay separate launches here."""
         g = self.grouping_cfg
-        dev = scores.device
-        base_radius = float(self._cfg(g, 'radius'))
         mean_active = int(self._cfg(g, 'mean_active'))
-        npoint_thr = float(self._cfg(g, 'npoint_thr'))
-        score_thr = float(self._cfg(g, 'score_thr'))
         with_pyramid = self._cfg(g, 'with_pyramid', False)
         with_octree = self._cfg(g, 'with_octree', False)
         base_size = self._cfg(g, 'pyramid_base_size', 0.02)
-        cnm = self._cfg(g, 'class_numpoint_mean')
-        ignore = set(self._cfg(g, 'ignore_classes', []))
-        min_npoint = int(self._cfg(self.test_cfg, 'min_npoint', 0))
         radius = base_radius
-        idx_list, off_list = [], []
-        n_prop, n_pts = 0, 0
-        for class_id in range(self.semantic_classes):
-            if class_id in ignore:
-                continue
+        parts = []
+        for class_id in classes:
             object_idxs = (scores[:, class_id] > score_thr).nonzero().view(-1)
             if object_idxs.size(0) < min_npoint:
                 continue
@@ -571,9 +564,7 @@ class SoftGroup(nn.Module):
             batch_offsets_ = self.get_batch_offsets(batch_idxs_, batch_size)
             neighbor_inds, start_len = ball_query((coords_ + pt_offsets_).contiguous(), batch_idxs_.contiguous(),
                                                   batch_offsets_, radius, mean_active, with_octree=with_octree)
-            thr = npoint_thr if cnm[class_id] == -1 else float(np.float32(npoint_thr) * np.float32(cnm[class_id]))
-            if neighbor_inds.numel() == 0:
-                neighbor_inds = torch.zeros(1, dtype=torch.int32, device=dev)
+            thr = functions.cluster_threshold(npoint_thr, cnm[class_id])
             pidx, poff = bfs_cluster_segments(neighbor_inds.contiguous(), start_len, thr)
             if l2p_map is not None:
                 pidx, poff = self.pyramid_inverse_map(pidx, poff, coords_.size(0), l2p_map)
@@ -581,14 +572,8 @@ class SoftGroup(nn.Module):
                 continue
             pidx = pidx.clone()
             pidx[:, 1] = object_idxs[pidx[:, 1].long()].int()
-            pidx[:, 0] += n_prop
-            idx_list.append(pidx)
-            off_list.append(poff[1:] + n_pts if off_list else poff)
-            n_prop += poff.numel() - 1
-            n_pts += pidx.size(0)
-        if not idx_list:
-            return (torch.zeros((0, 2), dtype=torch.int32, device=dev), torch.zeros((0, ), dtype=torch.int32, device=dev))
-        return torch.cat(idx_list, 0).contiguous(), torch.cat(off_list).int().contiguous()
+            parts.append((pidx, poff))
+        return _concat_proposals(parts, scores.device)
 
     def get_level(self, num_points):
         """softgroup.py:482-489."""

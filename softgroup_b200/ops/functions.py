@@ -16,6 +16,7 @@ Differences that are extensions, not changes:
 """
 import ctypes
 
+import numpy as np
 import torch
 from torch.autograd import Function
 
@@ -251,14 +252,25 @@ def group_entries(scores, classes, score_thr, min_npoint, batch_idxs, batch_size
 # ----------------------------------------------------------------------------------------------
 # clustering
 # ----------------------------------------------------------------------------------------------
+def cluster_threshold(npoint_thr, class_numpoint_mean):
+    """Smallest component size kept for one class (bfs_cluster.cpp:70-77 of the reference): npoint_thr * class mean
+    in float32 arithmetic like the C++ (`thr = threshold * _class_numpoint_mean`, both float), or npoint_thr itself
+    when the class mean is -1."""
+    if class_numpoint_mean == -1:
+        return float(npoint_thr)
+    return float(np.float32(npoint_thr) * np.float32(class_numpoint_mean))
+
+
 def bfs_cluster_segments(ball_query_idxs, start_len, thr, node_seg=None, seg_thr=None, nactive=None,
                          upstream_err=None):
-    """GPU clustering on device tensors. thr: float threshold on the component size (already multiplied by the
-    class mean when that applies). Optional per-node segment thresholds. Returns CUDA tensors
+    """GPU clustering on device tensors. thr: float threshold on the component size (cluster_threshold of the class).
+    Optional per-node segment thresholds. Returns CUDA tensors
     (cluster_idxs int32 [sumNPoint,2], cluster_offsets int32 [nCluster+1])."""
     L = _lib.lib()
     dev = start_len.device
     N = start_len.size(0)
+    if ball_query_idxs.numel() == 0:  # no neighbours at all: a one-word buffer, never read, in place of an empty one
+        ball_query_idxs = torch.zeros(1, dtype=torch.int32, device=dev)
     ws = _ws(L.sgb_bfs_cluster_workspace_bytes(N), dev)
     s = ctypes.c_int(0)
     mx = ctypes.c_int(0)
@@ -312,16 +324,9 @@ class BFSCluster(Function):
         assert cluster_numpoint_mean.is_contiguous()
         assert ball_query_idxs.is_contiguous()
         assert start_len.is_contiguous()
-        mean = float(cluster_numpoint_mean[class_id])
-        # float32 arithmetic like the C++ (`thr = threshold * _class_numpoint_mean`, both float)
-        thr = float(threshold) if mean == -1 else float(
-            torch.tensor(threshold, dtype=torch.float32) * torch.tensor(mean, dtype=torch.float32))
+        thr = cluster_threshold(threshold, float(cluster_numpoint_mean[class_id]))
         on_cpu = not ball_query_idxs.is_cuda
-        idxs = _cuda(ball_query_idxs)
-        sl = _cuda(start_len)
-        if idxs.numel() == 0:
-            idxs = torch.zeros(1, dtype=torch.int32, device=sl.device)
-        cidx, coff = bfs_cluster_segments(idxs, sl, thr)
+        cidx, coff = bfs_cluster_segments(_cuda(ball_query_idxs), _cuda(start_len), thr)
         if on_cpu:
             cidx, coff = cidx.cpu(), coff.cpu()
             if TORCH2_COMPAT:

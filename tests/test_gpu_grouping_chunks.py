@@ -7,6 +7,7 @@ list cursor addresses (2^31 - 1 / 1000 = 2,147,483 entries), forward_grouping cu
   * one segment alone beyond the bound: it runs when its neighbour total fits int32 and raises SgbError, without
     clustering, when it does not."""
 import itertools
+import warnings
 
 import numpy as np
 import pytest
@@ -67,6 +68,20 @@ def _patched(m, bound, planner):
         m.setattr(functions, 'plan_ballquery_chunks', planner)
 
 
+def _host_reads(model, *args):
+    """Synchronising CUDA operations torch sees in one forward_grouping, with batch_size given as forward_test gives it
+    (without it, forward_grouping reads the batch size back from the device)."""
+    prev = torch.cuda.get_sync_debug_mode()
+    try:
+        with warnings.catch_warnings(record=True) as seen, torch.no_grad():
+            warnings.simplefilter('always')
+            torch.cuda.set_sync_debug_mode('warn')
+            model.forward_grouping(*args, batch_size=1)
+    finally:
+        torch.cuda.set_sync_debug_mode(prev)
+    return sum('synchronizing CUDA operation' in str(w.message) for w in seen)
+
+
 def _same_instances(a, b):
     assert len(a) == len(b) and len(a) > 0
     for x, y in zip(a, b):
@@ -97,15 +112,22 @@ def test_forced_chunks_bit_identical(monkeypatch, case):
     hb = harness.to_host_batch(scan)
     with torch.no_grad():
         want_inst = harness.run_scan(model, hb, inject_pointwise=(scores, offs))['pred_instances']
+    # host reads after warm-up: below the bound only the entry count
+    assert _host_reads(model, *args) == 1
     for bound, planner in _forced(counts):
         with monkeypatch.context() as m:
             _patched(m, bound, planner)
             with torch.no_grad():
                 idx, off = model.forward_grouping(*args)
                 inst = harness.run_scan(model, hb, inject_pointwise=(scores, offs))['pred_instances']
+            reads = _host_reads(model, *args)
         assert np.array_equal(off.cpu().numpy(), want_off), (bound, planner)
         assert np.array_equal(idx.cpu().numpy(), want_idx), (bound, planner)
         _same_instances(inst, want_inst)
+        # beyond it also the segment offsets, and the flags of every range whose entries x 1000 exceed the bound
+        ranges = (planner or functions.plan_ballquery_chunks)(counts, bound)
+        oversize = sum(1 for s0, s1 in ranges if counts[s0:s1].sum() * 1000 > bound)
+        assert reads == 2 + oversize, (bound, planner, reads, oversize)
 
 
 # ---- beyond the bound, unpatched -------------------------------------------------------------------------------------
