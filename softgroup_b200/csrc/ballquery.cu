@@ -464,12 +464,23 @@ __global__ void __launch_bounds__(BqCfg<PASS>::kThreads, BqCfg<PASS>::kPerSM) bq
   }
 }
 
+static DeviceOnce g_bq_once;  // the query kernels' shared-memory attributes are set
+
 static int bq_launch(int n, long long capacity, float radius, const float *xyz, const int32_t *batch_idxs,
                      const int32_t *batch_offsets, int B, int32_t *idx, int32_t *start_len, void *ws, size_t ws_bytes,
                      cudaStream_t st, BqWs &w) {
   SGB_REQUIRE(n >= 0 && B >= 1 && B <= kMaxSeg && radius > 0.f, SGB_ERR_ARG, "ballquery arguments");
   SGB_REQUIRE(xyz && batch_idxs && batch_offsets && start_len && ws, SGB_ERR_ARG, "null pointer");
   SGB_REQUIRE(bq_carve(ws, ws_bytes, n, w), SGB_ERR_WORKSPACE, "ballquery workspace too small");
+  constexpr size_t smem0 = sizeof(float4) * BqCfg<0>::kSMax + 6 * BqCfg<0>::kBmWords;
+  constexpr size_t smem1 = sizeof(float4) * BqCfg<1>::kSMax + 6 * BqCfg<1>::kBmWords;
+  SGB_CURRENT_DEVICE(d);
+  int rc = once_per_device(g_bq_once, d->ordinal, [] {
+    SGB_CUDA_CHECK(cudaFuncSetAttribute(bq_query_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem0));
+    SGB_CUDA_CHECK(cudaFuncSetAttribute(bq_query_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
+    return SGB_OK;
+  });
+  if (rc) return rc;
   SGB_CUDA_CHECK(cudaMemsetAsync(w.keys, 0xFF, (size_t)w.cap * 8, st));
   SGB_CUDA_CHECK(cudaMemsetAsync(w.slot_cnt, 0, (size_t)w.cap * 4, st));
   SGB_CUDA_CHECK(cudaMemsetAsync(w.slot_fill, 0, (size_t)w.cap * 4, st));
@@ -482,26 +493,18 @@ static int bq_launch(int n, long long capacity, float radius, const float *xyz, 
   SGB_LAUNCH_CHECK();
   bq_cellcnt_kernel<<<nb, 256, 0, st>>>(n, w);
   SGB_LAUNCH_CHECK();
-  int rc = exclusive_scan_i32(w.cell_cnt, w.cell_cnt, (size_t)n, nullptr, w.scan_tmp, st);
+  rc = exclusive_scan_i32(w.cell_cnt, w.cell_cnt, (size_t)n, nullptr, w.scan_tmp, st);
   if (rc) return rc;
   bq_cellstart_kernel<<<nb, 256, 0, st>>>(n, w);
   SGB_LAUNCH_CHECK();
   bq_scatter_kernel<<<nb, 256, 0, st>>>(xyz, n, w);
   SGB_LAUNCH_CHECK();
-  constexpr size_t smem0 = sizeof(float4) * BqCfg<0>::kSMax + 6 * BqCfg<0>::kBmWords;
-  constexpr size_t smem1 = sizeof(float4) * BqCfg<1>::kSMax + 6 * BqCfg<1>::kBmWords;
-  static bool attr_set = false;
-  if (!attr_set) {
-    SGB_CUDA_CHECK(cudaFuncSetAttribute(bq_query_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem0));
-    SGB_CUDA_CHECK(cudaFuncSetAttribute(bq_query_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-    attr_set = true;
-  }
-  bq_query_kernel<0><<<std::min(std::max(n, 1), BqCfg<0>::kPerSM * kNumSMs), BqCfg<0>::kThreads, smem0, st>>>(
+  bq_query_kernel<0><<<std::min(std::max(n, 1), BqCfg<0>::kPerSM * d->sms), BqCfg<0>::kThreads, smem0, st>>>(
       xyz, batch_idxs, batch_offsets, n, radius, capacity, idx, start_len, w);
   SGB_LAUNCH_CHECK();
   // the items pass 0 noted (stencils of up to 10240 candidates stay on the staged path; beyond that the exact scan)
-  bq_query_kernel<1><<<std::min(std::max(n, 1), kNumSMs), BqCfg<1>::kThreads, smem1, st>>>(xyz, batch_idxs, batch_offsets, n, radius,
-                                                                                         capacity, idx, start_len, w);
+  bq_query_kernel<1><<<std::min(std::max(n, 1), d->sms), BqCfg<1>::kThreads, smem1, st>>>(xyz, batch_idxs, batch_offsets, n, radius,
+                                                                                        capacity, idx, start_len, w);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

@@ -481,6 +481,11 @@ __global__ void __cluster_dims__(kCl, 1, 1) __launch_bounds__(kClThreads)
   }
 }
 
+// as many 8-CTA emit2 clusters as a device keeps resident at once (several CTAs per SM: the kernel is latency bound on
+// its per-level cluster barriers, so components in flight -- not threads per component -- is what fills the machine)
+static DeviceOnce g_emit2_once;
+static int g_emit2_clusters[kMaxDevices];
+
 }  // namespace sgb
 
 using namespace sgb;
@@ -506,11 +511,12 @@ int sgb_bfs_cluster_count(const int32_t *d_ball_query_idxs, const int32_t *d_sta
   SGB_REQUIRE((d_node_seg == nullptr) == (d_seg_thr == nullptr), SGB_ERR_ARG, "node_seg / seg_thr must come together");
   BfsWs w;
   SGB_REQUIRE(bfs_carve(d_ws, ws_bytes, N, w), SGB_ERR_WORKSPACE, "bfs_cluster workspace too small");
+  SGB_CURRENT_DEVICE(d);
   int nb = div_up(N, 256);
   SGB_CUDA_CHECK(cudaMemsetAsync(w.scalars, 0, 64 * 4, st));
   bfs_init_kernel<<<nb, 256, 0, st>>>(N, w);
   SGB_LAUNCH_CHECK();
-  int grid = std::min(div_up((long long)N * 32, 256), kNumSMs * 16);
+  int grid = std::min(div_up((long long)N * 32, 256), d->sms * 16);
   // passes in batches of kBatch launches, ONE host synchronisation per batch (the one that reads the cluster totals):
   // sizes / threshold / scan are enqueued optimistically behind the batch and redone in the rare case that the last
   // pass of the batch still pushed labels (flags live in scalars[8..8+kBatch)).
@@ -578,22 +584,21 @@ int sgb_bfs_cluster_fill(const int32_t *d_ball_query_idxs, const int32_t *d_star
     SGB_CUDA_CHECK(cudaMemsetAsync(w.cursor, 0, (size_t)nCluster * 4, st));
     bfs_members_kernel<<<nb, 256, 0, st>>>(N, d_cluster_offsets, w);
     SGB_LAUNCH_CHECK();
-    // as many 8-CTA clusters as the device keeps resident at once (several CTAs per SM: the kernel is latency bound on its
-    // per-level cluster barriers, so components in flight -- not threads per component -- is what fills the machine)
-    static int max_clusters = 0;
-    if (!max_clusters) {
+    SGB_CURRENT_DEVICE(d);
+    once_per_device(g_emit2_once, d->ordinal, [d] {
       cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(kNumSMs * 4 / kCl * kCl);
+      cfg.gridDim = dim3(d->sms * 4 / kCl * kCl);
       cfg.blockDim = dim3(kClThreads);
       cudaLaunchAttribute attr[1];
       attr[0].id = cudaLaunchAttributeClusterDimension;
       attr[0].val.clusterDim.x = kCl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
       cfg.attrs = attr; cfg.numAttrs = 1;
       int n = 0;
-      if (cudaOccupancyMaxActiveClusters(&n, bfs_emit2_kernel, &cfg) != cudaSuccess || n < 1) { cudaGetLastError(); n = kNumSMs / kCl; }
-      max_clusters = n;
-    }
-    int n_cl = std::min(nCluster, max_clusters);
+      if (cudaOccupancyMaxActiveClusters(&n, bfs_emit2_kernel, &cfg) != cudaSuccess || n < 1) { cudaGetLastError(); n = d->sms / kCl; }
+      g_emit2_clusters[d->ordinal] = n;
+      return SGB_OK;
+    });
+    int n_cl = std::min(nCluster, g_emit2_clusters[d->ordinal]);
     bfs_emit2_kernel<<<n_cl * kCl, kClThreads, 0, st>>>(d_ball_query_idxs, d_start_len, d_cluster_offsets, d_cluster_idxs,
                                                        nCluster, W, (uint32_t *)d_scratch, w);
     SGB_LAUNCH_CHECK();

@@ -4,6 +4,9 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <atomic>
+#include <mutex>
+
 #include "../../include/sgb200.h"
 
 namespace sgb {
@@ -34,7 +37,35 @@ void count_launch();  // bumps the process-wide kernel-launch counter (sgb_launc
     }                                                                \
   } while (0)
 
-constexpr int kNumSMs = 132;  // H100 SXM (the launch code asks the device where it can)
+// Per-device launch state, built on a device's first use, once, thread-safely. Grids that cover the machine are sized
+// from `sms`.
+constexpr int kMaxDevices = 16;
+
+struct Device {
+  int ordinal;
+  int sms;     // multiprocessors
+  int *oflow;  // flag raised by the packing code when a value leaves the fp16 range (sgb_spconv_overflow)
+};
+
+// The current device's record (errors through set_error). SGB_CURRENT_DEVICE(d) declares `Device *d` or returns the error.
+int current_device(Device **d);
+#define SGB_CURRENT_DEVICE(d) \
+  sgb::Device *d;             \
+  if (const int _rc = sgb::current_device(&d)) return _rc
+
+// One-time set-up of a module, per device: init() runs until it first returns SGB_OK, then never again. A failed
+// init has reported its error on the calling thread, and the next call tries again.
+struct DeviceOnce { std::atomic<bool> done[kMaxDevices] = {}; std::mutex m; };
+
+template <typename F>
+int once_per_device(DeviceOnce &once, int dev, F &&init) {
+  if (once.done[dev].load(std::memory_order_acquire)) return SGB_OK;
+  std::lock_guard<std::mutex> lock(once.m);
+  if (once.done[dev].load(std::memory_order_relaxed)) return SGB_OK;
+  const int rc = init();
+  if (rc == SGB_OK) once.done[dev].store(true, std::memory_order_release);
+  return rc;
+}
 
 static inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 static inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }

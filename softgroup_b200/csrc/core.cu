@@ -1,6 +1,5 @@
-// core.cu -- error reporting, device probe, device-wide exclusive scan.
+// core.cu -- error reporting, device probe, per-device launch state, device-wide exclusive scan.
 #include <stdarg.h>
-#include <atomic>
 #include <string.h>
 
 #include "common.cuh"
@@ -17,6 +16,28 @@ void set_error(const char *fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
+}
+
+static Device g_devices[kMaxDevices];
+static DeviceOnce g_devices_once;
+
+int current_device(Device **out) {
+  int dev;
+  SGB_CUDA_CHECK(cudaGetDevice(&dev));
+  SGB_REQUIRE(dev >= 0 && dev < kMaxDevices, SGB_ERR_RANGE, "device ordinal beyond 15");
+  Device &d = g_devices[dev];
+  int rc = once_per_device(g_devices_once, dev, [&] {
+    d.ordinal = dev;
+    SGB_CUDA_CHECK(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
+    SGB_CUDA_CHECK(cudaMalloc(&d.oflow, 4));
+    SGB_CUDA_CHECK(cudaMemset(d.oflow, 0, 4));
+    // the zero must land before any stream's kernel can raise the flag: the scan streams do not wait for the default one
+    SGB_CUDA_CHECK(cudaStreamSynchronize(0));
+    return SGB_OK;
+  });
+  if (rc) return rc;
+  *out = &d;
+  return SGB_OK;
 }
 
 constexpr int kScanThreads = 512;

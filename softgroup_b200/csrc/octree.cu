@@ -236,8 +236,9 @@ long long sgb_octree_ball_query(const float *d_points, const float *d_boxes, con
   if (n == 0) return 0;
   SGB_REQUIRE(d_points && d_boxes && d_pt_inds && d_pt_start_len && d_out_start_len && d_total && mean_active >= 0,
               SGB_ERR_ARG, "octree_ball_query arguments");
+  SGB_CURRENT_DEVICE(d);
   SGB_CUDA_CHECK(cudaMemsetAsync(d_total, 0, 4, st));
-  int grid = std::min(div_up(n, OQ_WARPS), kNumSMs * 4);
+  int grid = std::min(div_up(n, OQ_WARPS), d->sms * 4);
   oc_query_kernel<<<grid, OQ_WARPS * 32, 0, st>>>(d_points, d_boxes, d_pt_inds, d_pt_start_len, n, radius,
                                                  (long long)n * mean_active, d_out_inds, d_out_start_len, d_total);
   SGB_LAUNCH_CHECK();

@@ -241,11 +241,12 @@ static int seg_launch(const float *inp, const int32_t *off, float *out, int nP, 
   if (nP == 0 || C == 0) return SGB_OK;
   SGB_REQUIRE(inp && off && out && nP > 0 && C > 0, SGB_ERR_ARG, "segment reduce arguments");
   if (OP == OP_MIN || OP == OP_MAX) {
+    SGB_CURRENT_DEVICE(d);
     // an empty proposal keeps the initial value: +inf / -inf, what `1e50` / `-1e50` become as float (sec_mean.cu:47,73)
     const long long n = (long long)nP * C;
     seg_fill_kernel<<<div_up(n, 256), 256, 0, (cudaStream_t)stream>>>(out, n, OP == OP_MIN ? INFINITY : -INFINITY);
     SGB_LAUNCH_CHECK();
-    seg_minmax_kernel<OP><<<kNumSMs * 4, kSegThreads, 0, (cudaStream_t)stream>>>(inp, off, out, nP, C, pow2_cw(C));
+    seg_minmax_kernel<OP><<<d->sms * 4, kSegThreads, 0, (cudaStream_t)stream>>>(inp, off, out, nP, C, pow2_cw(C));
     SGB_LAUNCH_CHECK();
     return SGB_OK;
   }

@@ -328,29 +328,11 @@ using namespace sgb;
 
 namespace {
 
-int *g_oflow[16] = {nullptr};  // per device: flag raised by the packing code when a value leaves the fp16 range
+constexpr int kNumSMs = 132;  // H100 SXM: what the pure plan functions assume when the caller gives no SM count
 
-struct DevInfo { int sms; bool attr_set[9]; int per_sm[9]; };  // per NT / 16: shared-memory attribute set, CTAs per SM
-DevInfo g_dev[16] = {};
-
-int current_device(int *dev) {
-  SGB_CUDA_CHECK(cudaGetDevice(dev));
-  SGB_REQUIRE(*dev >= 0 && *dev < 16, SGB_ERR_RANGE, "device ordinal beyond 15");
-  return SGB_OK;
-}
-
-int ensure_device(int dev) {
-  if (!g_dev[dev].sms) {
-    int sms = 0;
-    SGB_CUDA_CHECK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    g_dev[dev].sms = sms;
-  }
-  if (!g_oflow[dev]) {
-    SGB_CUDA_CHECK(cudaMalloc(&g_oflow[dev], 4));
-    SGB_CUDA_CHECK(cudaMemset(g_oflow[dev], 0, 4));
-  }
-  return SGB_OK;
-}
+// per NT / 16: the kernel's shared-memory attribute is set and its CTAs per SM are known, per device
+DeviceOnce g_tc_once[9];
+int g_tc_per_sm[kMaxDevices][9];
 
 // Columns per work item of the persistent launch: all of N up to 128, else N cut into equal parts (multiple of 16).
 int persistent_nt(int N) { return N <= 128 ? N : (div_up(N, div_up(N, 128)) + 15) / 16 * 16; }
@@ -368,18 +350,19 @@ bool use_persistent(int K, int Mout, int Cin, int Cout, int sms) {
 }
 
 template <int NT>
-int launch_nt(const TcArgs &p, bool persistent, int dev, cudaStream_t stream) {
+int launch_nt(const TcArgs &p, bool persistent, const Device &d, cudaStream_t stream) {
   const size_t smem = tc_smem_bytes(NT);
-  DevInfo &d = g_dev[dev];
-  if (!d.attr_set[NT / 16]) {
+  int *per_sm = &g_tc_per_sm[d.ordinal][NT / 16];
+  int rc = once_per_device(g_tc_once[NT / 16], d.ordinal, [&] {
     SGB_CUDA_CHECK(cudaFuncSetAttribute(spconv_tc_kernel<NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int n = 0;
     SGB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, spconv_tc_kernel<NT>, TC_THREADS, smem));
-    d.per_sm[NT / 16] = std::max(n, 1);
-    d.attr_set[NT / 16] = true;
-  }
+    *per_sm = std::max(n, 1);
+    return SGB_OK;
+  });
+  if (rc) return rc;
   if (persistent) {
-    const int grid = std::min(p.items, d.sms * d.per_sm[NT / 16]);
+    const int grid = std::min(p.items, d.sms * *per_sm);
     spconv_tc_kernel<NT><<<grid, TC_THREADS, smem, stream>>>(p);
   } else if (p.ksplit == 1) {
     spconv_tc_kernel<NT><<<p.items, TC_THREADS, smem, stream>>>(p);
@@ -402,16 +385,16 @@ int launch_nt(const TcArgs &p, bool persistent, int dev, cudaStream_t stream) {
   return SGB_OK;
 }
 
-int launch(int NT, const TcArgs &p, bool persistent, int dev, cudaStream_t stream) {
+int launch(int NT, const TcArgs &p, bool persistent, const Device &d, cudaStream_t stream) {
   switch (NT) {
-    case 16: return launch_nt<16>(p, persistent, dev, stream);
-    case 32: return launch_nt<32>(p, persistent, dev, stream);
-    case 48: return launch_nt<48>(p, persistent, dev, stream);
-    case 64: return launch_nt<64>(p, persistent, dev, stream);
-    case 80: return launch_nt<80>(p, persistent, dev, stream);
-    case 96: return launch_nt<96>(p, persistent, dev, stream);
-    case 112: return launch_nt<112>(p, persistent, dev, stream);
-    case 128: return launch_nt<128>(p, persistent, dev, stream);
+    case 16: return launch_nt<16>(p, persistent, d, stream);
+    case 32: return launch_nt<32>(p, persistent, d, stream);
+    case 48: return launch_nt<48>(p, persistent, d, stream);
+    case 64: return launch_nt<64>(p, persistent, d, stream);
+    case 80: return launch_nt<80>(p, persistent, d, stream);
+    case 96: return launch_nt<96>(p, persistent, d, stream);
+    case 112: return launch_nt<112>(p, persistent, d, stream);
+    case 128: return launch_nt<128>(p, persistent, d, stream);
   }
   SGB_REQUIRE(false, SGB_ERR_RANGE, "spconv_forward_tc: columns per CTA not a multiple of 16 in [16, 128]");
 }
@@ -427,14 +410,11 @@ int sgb_spconv_lo_shift(void) { return sgb::kLoShift; }
 int sgb_spconv_overflow(int *h_flag, void *stream) {
   SGB_REQUIRE(h_flag, SGB_ERR_ARG, "null flag");
   *h_flag = 0;
-  int dev;
-  int rc = current_device(&dev);
-  if (rc) return rc;
-  if (!g_oflow[dev]) return SGB_OK;
+  SGB_CURRENT_DEVICE(d);
   cudaStream_t st = (cudaStream_t)stream;
-  SGB_CUDA_CHECK(cudaMemcpyAsync(h_flag, g_oflow[dev], 4, cudaMemcpyDeviceToHost, st));
+  SGB_CUDA_CHECK(cudaMemcpyAsync(h_flag, d->oflow, 4, cudaMemcpyDeviceToHost, st));
   SGB_CUDA_CHECK(cudaStreamSynchronize(st));
-  if (*h_flag) SGB_CUDA_CHECK(cudaMemsetAsync(g_oflow[dev], 0, 4, st));
+  if (*h_flag) SGB_CUDA_CHECK(cudaMemsetAsync(d->oflow, 0, 4, st));
   return SGB_OK;
 }
 
@@ -444,14 +424,10 @@ int sgb_act_pack(const float *d_x, int x_stride, int x_off, const float *d_scale
   SGB_REQUIRE(d_x && d_pk && M > 0 && C > 0 && (d_scale == nullptr) == (d_shift == nullptr), SGB_ERR_ARG, "act_pack arguments");
   SGB_REQUIRE((pk_stride & 31) == 0 && (pk_coff & 1) == 0 && (Cfill & 1) == 0 && Cfill >= C && pk_stride >= pk_coff + Cfill,
               SGB_ERR_ARG, "act_pack: row stride multiple of 32 words, channel offset and fill width even, fill inside the row");
-  int dev;
-  int rc = current_device(&dev);
-  if (rc) return rc;
-  rc = ensure_device(dev);
-  if (rc) return rc;
+  SGB_CURRENT_DEVICE(d);
   long long tot = (long long)M * (Cfill / 2);
   act_pack_kernel<<<div_up(tot, 256), 256, 0, (cudaStream_t)stream>>>(d_x, x_stride, x_off, d_scale, d_shift, relu,
-                                                                    (uint32_t *)d_pk, pk_stride, pk_coff, M, C, Cfill, g_oflow[dev]);
+                                                                    (uint32_t *)d_pk, pk_stride, pk_coff, M, C, Cfill, d->oflow);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }
@@ -525,12 +501,8 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
   SGB_REQUIRE((d_pk_scale == nullptr) == (d_pk_shift == nullptr), SGB_ERR_ARG, "scale/shift must come together");
   const int N = (Cout + 15) / 16 * 16;
   SGB_REQUIRE(N <= 256 && Cin <= 512, SGB_ERR_RANGE, "spconv_forward_tc: Cout > 256 or Cin > 512 is not tiled");
-  int dev;
-  int rc = current_device(&dev);
-  if (rc) return rc;
-  rc = ensure_device(dev);
-  if (rc) return rc;
-  const bool persistent = kernel == 1 || (kernel == -1 && use_persistent(K, Mout, Cin, Cout, g_dev[dev].sms));
+  SGB_CURRENT_DEVICE(d);
+  const bool persistent = kernel == 1 || (kernel == -1 && use_persistent(K, Mout, Cin, Cout, d->sms));
   TcArgs p;
   p.in = (const uint32_t *)d_in_pk; p.in_stride = in_stride;
   p.map = d_map; p.K = K; p.Mout = Mout;
@@ -540,7 +512,7 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
   p.out = d_out; p.out_stride = out_stride; p.out_off = out_off;
   p.pk = (uint32_t *)d_pk_out; p.pk_stride = pk_stride; p.pk_coff = pk_coff;
   p.pk_scale = d_pk_scale; p.pk_shift = d_pk_shift; p.pk_relu = pk_relu; p.pk_fill = pk_fill;
-  p.oflow = g_oflow[dev];
+  p.oflow = d->oflow;
   const int tiles = div_up(Mout, TC_ROWS);
   int NT;
   if (persistent) {
@@ -548,13 +520,13 @@ int sgb_spconv_forward_tc_ex(const float *d_in_pk, int in_stride, int Min, const
     p.ksplit = 1;
   } else {
     int plan[6];
-    rc = sgb_spconv_tc_plan(K, Mout, Cin, Cout, d_map != nullptr, g_dev[dev].sms, plan);
+    int rc = sgb_spconv_tc_plan(K, Mout, Cin, Cout, d_map != nullptr, d->sms, plan);
     if (rc) return rc;
     NT = plan[0];
     p.ksplit = plan[2];
   }
   p.nparts = div_up(N, NT);
   p.items = tiles * p.nparts;
-  return launch(NT, p, persistent, dev, (cudaStream_t)stream);
+  return launch(NT, p, persistent, *d, (cudaStream_t)stream);
 }
 }

@@ -200,8 +200,7 @@ def transform_test_gpu(xyz, scale, x4_split=False):
     N = xyz.size(0)
     m = np.ascontiguousarray(_test_rotation(), dtype=np.float64)
     mid = torch.empty((N, 3), dtype=torch.float64, device=xyz.device)
-    check(_lib.lib().sgb_affine3_f64(ptr(xyz), m.ctypes.data_as(ctypes.c_void_p), ptr(mid), N,
-                                     ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'sgb_affine3_f64')
+    check(_lib.lib().sgb_affine3_f64(ptr(xyz), m.ctypes.data_as(ctypes.c_void_p), ptr(mid), N, _lib.stream()), 'sgb_affine3_f64')
     if not x4_split:
         s = mid * float(scale)
         s = s - s.min(0)[0]

@@ -400,7 +400,6 @@ class SoftGroup(nn.Module):
         else:
             from ..ops import _lib
             from ..ops._lib import check, ptr
-            import ctypes
             vf = self._run_stack('backbone', self.input_conv, self.unet, self.output_layer, input)
             if vf.stride(0) != vf.size(1):
                 vf = vf.contiguous()
@@ -409,9 +408,8 @@ class SoftGroup(nn.Module):
             # output_feats[input_map.long()] (:374) -- the "devoxelize" gather
             from .. import profiler
             with profiler.record('gather_rows(devoxelize)', 4 * N + 4 * vf.size(1) * (vf.size(0) + N)):
-                check(_lib.lib().sgb_gather_rows(ptr(vf), ptr(input_map.contiguous()), ptr(output_feats), N,
-                                                 vf.size(1), ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)),
-                      'sgb_gather_rows')
+                check(_lib.lib().sgb_gather_rows(ptr(vf), ptr(input_map.contiguous()), ptr(output_feats), N, vf.size(1),
+                                                 _lib.stream()), 'sgb_gather_rows')
         semantic_scores = self.semantic_linear(output_feats)
         pt_offsets = self.offset_linear(output_feats)
         return semantic_scores, pt_offsets, output_feats

@@ -198,7 +198,7 @@ class Plan(object):
         c_subm, c_down, c_inv = (ctypes.c_void_p * L)(), (ctypes.c_void_p * L)(), (ctypes.c_void_p * L)()
         c_M = (ctypes.c_int * L)()
         c_bufs[self.in_buf] = ptrs[self.in_buf]
-        stream = core._stream()
+        stream = _lib.stream()
         op_size = ctypes.sizeof(UnetOp)
         for (i0, i1, need) in self.segments:
             while opened < need:

@@ -8,6 +8,8 @@ import ctypes
 import os
 from ctypes import c_double, c_float, c_int, c_longlong, c_size_t, c_void_p
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(os.path.dirname(_HERE), 'libsgb200.so')
 
@@ -116,3 +118,17 @@ def check(rc, what=''):
 def ptr(t):
     """Device/host pointer of a tensor (None -> NULL)."""
     return None if t is None else c_void_p(t.data_ptr())
+
+
+def stream():
+    """Handle of torch's current CUDA stream, the `stream` argument of every entry point."""
+    # the raw-handle call avoids ~10 us of Python per launch
+    try:
+        return c_void_p(torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice()))
+    except Exception:  # older torch: public (slower) path
+        return c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def workspace(nbytes, device):
+    """Uninitialised device scratch of `nbytes` bytes (the `d_ws` / `d_scratch` arguments)."""
+    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)

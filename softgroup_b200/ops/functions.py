@@ -22,19 +22,7 @@ from torch.autograd import Function
 
 from .. import profiler
 from . import _lib
-from ._lib import check, ptr
-
-
-def _stream():
-    # raw handle of torch's current stream; the C entry point avoids ~10 us of Python per launch
-    try:
-        return ctypes.c_void_p(torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice()))
-    except Exception:  # older torch: public (slower) path
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _ws(nbytes, device):
-    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+from ._lib import check, ptr, stream as _stream, workspace as _ws
 
 
 def _cuda(t):

@@ -9,15 +9,7 @@ import torch
 
 from .. import profiler
 from . import _lib
-from ._lib import check, ptr
-
-
-def _stream():
-    return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _ws(nbytes, device):
-    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
+from ._lib import check, ptr, stream as _stream, workspace as _ws
 
 
 def bitmap_words(n_points):

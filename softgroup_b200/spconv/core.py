@@ -20,15 +20,7 @@ from torch import nn
 
 from .. import profiler
 from ..ops import _lib
-from ..ops._lib import check, ptr
-
-
-def _stream():
-    # raw handle of torch's current stream; the C entry point avoids ~10 us of Python per launch
-    try:
-        return ctypes.c_void_p(torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice()))
-    except Exception:  # older torch: public (slower) path
-        return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+from ..ops._lib import check, ptr, stream as _stream, workspace as _ws
 
 
 class SparseConvTensor(object):
@@ -103,10 +95,6 @@ def bn_relu_rows(x, scale, shift, relu):
 # ---------------------------------------------------------------------------------------------------------
 # rulebooks
 # ---------------------------------------------------------------------------------------------------------
-def _ws(nbytes, device):
-    return torch.empty(int(nbytes), dtype=torch.uint8, device=device)
-
-
 def _indices_i32(indices):
     if indices.dtype != torch.int32:
         indices = indices.int()

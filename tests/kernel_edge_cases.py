@@ -9,7 +9,7 @@ import numpy as np
 # launch constants of softgroup_b200/csrc
 SEG_THREADS = 256  # segment.cu kSegThreads
 SEG_CHUNK = 2048  # segment.cu kSegChunk: min / max partials are per 2048-row chunk
-SEG_GRID = 132 * 4  # seg_minmax_kernel grid (kNumSMs * 4): more than SEG_GRID chunks take the grid-stride loop
+SEG_GRID = 132 * 4  # seg_minmax_kernel grid (SMs * 4, H100 SXM): more than SEG_GRID chunks take the grid-stride loop
 MEAN_GRID = 65535  # seg_reduce_kernel / avg_pool_bp_kernel grid cap: more proposals take the grid-stride loop
 SCAN_TILE = 512 * 8  # core.cu kScanTile: exclusive_scan_i32 has 2 levels above one tile, 3 above SCAN_TILE**2
 PAN_THREADS = 1024  # instances.cu kPanThreads: one CTA walks the words of a mask
