@@ -52,7 +52,7 @@ int sgb_device_available(void);
  * mode: 0 unique, 1 first, 2 last, 3 sum, 4 mean (only the map differs; 4 is what the model uses).
  *
  * GPU path: keys are packed into 64 bits: batch in [0, 65535], x,y,z in [-32768, 32767]
- * (all reference configs fit); anything outside returns SGB_ERR_RANGE.
+ * (all reference configs fit, the corners included); anything outside returns SGB_ERR_RANGE.
  *   count (blocking): fills d_input_map [N]; returns M and maxActive through h_M / h_maxActive.
  *   fill: d_output_coords int64 [M, ncol], d_output_map int32 [M, maxActive+1]. Must be called with
  *         the SAME workspace contents left by count.
@@ -184,11 +184,15 @@ int sgb_get_mask_label(const int32_t *d_proposals_idx, const int32_t *d_proposal
  * or -1. Kernel offset order = row-major (k0,k1,k2) like the weight layout [out,k0,k1,k2,in]
  * (tools/convert_checkpoint.py:17-19).
  *   subm3:   K=27, Mout=M, map[k][j] = row of indices[j] + (k0-1,k1-1,k2-1)           (SubMConv3d k3 p1)
+ *            subm3 does not report rows outside the range above: its callers pass indices that voxelize_idx or
+ *            down2 have already checked, and reporting would cost a host wait per level. Such a row is nobody's
+ *            neighbour, and its own map column holds only its centre entry (map[13][j] = j), -1 elsewhere.
  *   down2:   K=8; output voxels = distinct (b, x>>1, y>>1, z>>1) with every coordinate < out_shape
  *            = floor(shape/2) (inputs on the max plane of an odd dim are dropped), numbered by first
  *            occurrence in input order. count (blocking) returns Mout; fill writes d_out_indices [Mout,4],
  *            d_map [8,Mout] (children) and d_inv_map [8,M] (inv_map[k][i] = parent row if input i is child k
- *            of it, else -1) -- the inverse conv is the same kernel run with inv_map.   (SparseConv3d k2 s2,
+ *            of it, else -1) -- the inverse conv is the same kernel run with inv_map. With Mout = 0 (an axis of
+ *            extent 1) d_out_indices and d_map may be NULL.                          (SparseConv3d k2 s2,
  *            SparseInverseConv3d k2)
  * ------------------------------------------------------------------------------------------- */
 size_t sgb_rulebook_workspace_bytes(int M);

@@ -26,6 +26,8 @@ def _pack(idx):
 
 
 def _lookup(keys_sorted, order, q):
+    if len(keys_sorted) == 0:  # e.g. a down2 level without parents
+        return np.full(len(q), -1, np.int64)
     pos = np.searchsorted(keys_sorted, q)
     pos = np.clip(pos, 0, len(keys_sorted) - 1)
     hit = keys_sorted[pos] == q

@@ -105,7 +105,8 @@ __device__ __forceinline__ uint32_t hash64(unsigned long long k) {
   return (uint32_t)k;
 }
 
-// Insert-or-find; returns the slot. cap_mask = capacity-1 (capacity is a power of two >= 2*#keys).
+// Insert-or-find; returns the slot. cap_mask = capacity-1 (capacity is a power of two >= 2*#keys). key must not be
+// kEmptyKey: that key "finds" the first empty slot without claiming it.
 __device__ __forceinline__ uint32_t hash_insert(unsigned long long *keys, uint32_t cap_mask, unsigned long long key) {
   uint32_t s = hash64(key) & cap_mask;
   while (true) {

@@ -65,7 +65,7 @@ __global__ void rb_subm3_kernel(const int32_t *__restrict__ indices, int M, int3
   int dx = k / 9 - 1, dy = (k / 3) % 3 - 1, dz = k % 3 - 1;
   int r = -1;
   if (k == 13) r = j;
-  else {
+  else if (idx_ok(c.x, c.y, c.z, c.w)) {  // a rejected row's key could alias another row or equal kEmptyKey
     uint32_t s = hash_find(w.keys, w.cap - 1, vkey(c.x, c.y + dx, c.z + dy, c.w + dz));
     if (s != 0xFFFFFFFFu) r = w.vals[s];
   }
@@ -291,7 +291,9 @@ int sgb_rulebook_down2_fill(const int32_t *d_indices, int M, int Mout, int32_t *
                             int32_t *d_inv_map, void *d_ws, size_t ws_bytes, void *stream) {
   cudaStream_t st = (cudaStream_t)stream;
   if (M == 0) return SGB_OK;
-  SGB_REQUIRE(d_indices && d_out_indices && d_map && d_inv_map && d_ws, SGB_ERR_ARG, "rulebook_down2_fill arguments");
+  // with no parents (an axis of extent 1) the outputs of Mout rows are empty and may be null
+  SGB_REQUIRE(d_indices && (Mout == 0 || (d_out_indices && d_map)) && d_inv_map && d_ws, SGB_ERR_ARG,
+              "rulebook_down2_fill arguments");
   SGB_REQUIRE(((uintptr_t)d_out_indices & 15) == 0, SGB_ERR_ARG, "out_indices must be 16-byte aligned");
   RbWs w;
   SGB_REQUIRE(rb_carve(d_ws, ws_bytes, M, w), SGB_ERR_WORKSPACE, "rulebook workspace too small");

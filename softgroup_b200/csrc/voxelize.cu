@@ -26,13 +26,15 @@ __device__ __forceinline__ bool pack_key(const long long *c, int ncol, unsigned 
   return ok;
 }
 
+// The point (65535, 32767, 32767, 32767) packs to kEmptyKey, which the table cannot hold: its points skip the table
+// and share the reserved slot `cap` of the per-slot arrays.
 struct VoxWs {
   unsigned long long *keys;  // [cap]
-  int32_t *first;            // [cap] min point index of the slot
-  int32_t *last;             // [cap] max point index
-  int32_t *cnt;              // [cap]
-  int32_t *vid;              // [cap] voxel id of slot
-  int32_t *slot_of;          // [N]
+  int32_t *first;            // [cap + 1] min point index of the slot
+  int32_t *last;             // [cap + 1] max point index
+  int32_t *cnt;              // [cap + 1]
+  int32_t *vid;              // [cap + 1] voxel id of slot
+  int32_t *slot_of;          // [N] slot of the point, -1 for a point outside the key range
   int32_t *rank;             // [N] flags -> exclusive scan
   int32_t *fill;             // [N] (>= M) per-voxel fill cursor
   int32_t *scalars;          // [8]: 0 = M, 1 = maxActive, 2 = range error flag
@@ -47,10 +49,10 @@ static bool vox_carve(void *ws, size_t bytes, int N, VoxWs &w) {
   w.cap = (uint32_t)vox_cap(N);
   w.scalars = a.take<int32_t>(64);
   w.keys = a.take<unsigned long long>(w.cap);
-  w.first = a.take<int32_t>(w.cap);
-  w.last = a.take<int32_t>(w.cap);
-  w.cnt = a.take<int32_t>(w.cap);
-  w.vid = a.take<int32_t>(w.cap);
+  w.first = a.take<int32_t>((size_t)w.cap + 1);
+  w.last = a.take<int32_t>((size_t)w.cap + 1);
+  w.cnt = a.take<int32_t>((size_t)w.cap + 1);
+  w.vid = a.take<int32_t>((size_t)w.cap + 1);
   w.slot_of = a.take<int32_t>((size_t)N + 1);
   w.rank = a.take<int32_t>((size_t)N + 1);
   w.fill = a.take<int32_t>((size_t)N + 1);
@@ -62,8 +64,8 @@ __global__ void vox_insert_kernel(const long long *__restrict__ coords, int N, i
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   unsigned long long key;
-  if (!pack_key(coords + (size_t)i * ncol, ncol, key)) { w.scalars[2] = 1; return; }
-  uint32_t s = hash_insert(w.keys, w.cap - 1, key);
+  if (!pack_key(coords + (size_t)i * ncol, ncol, key)) { w.scalars[2] = 1; w.slot_of[i] = -1; return; }
+  uint32_t s = (key == kEmptyKey) ? w.cap : hash_insert(w.keys, w.cap - 1, key);
   w.slot_of[i] = (int32_t)s;
   atomicMin(&w.first[s], i);
   atomicMax(&w.last[s], i);
@@ -73,7 +75,8 @@ __global__ void vox_insert_kernel(const long long *__restrict__ coords, int N, i
 __global__ void vox_flag_kernel(int N, VoxWs w) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  w.rank[i] = (w.first[w.slot_of[i]] == i) ? 1 : 0;
+  int s = w.slot_of[i];
+  w.rank[i] = (s >= 0 && w.first[s] == i) ? 1 : 0;
 }
 
 // after the scan: rank[i] = voxel id for first-occurrence points
@@ -81,7 +84,7 @@ __global__ void vox_assign_kernel(int N, int mode, VoxWs w) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
   int s = w.slot_of[i];
-  if (w.first[s] == i) {
+  if (s >= 0 && w.first[s] == i) {
     w.vid[s] = w.rank[i];
     int c = (mode == 3 || mode == 4) ? w.cnt[s] : 1;
     // filtered atomic: only rows that beat the (possibly stale) running maximum touch the counter
@@ -92,7 +95,8 @@ __global__ void vox_assign_kernel(int N, int mode, VoxWs w) {
 __global__ void vox_inputmap_kernel(int N, int32_t *__restrict__ input_map, VoxWs w) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= N) return;
-  input_map[i] = w.vid[w.slot_of[i]];
+  int s = w.slot_of[i];
+  input_map[i] = (s >= 0) ? w.vid[s] : -1;
 }
 
 __global__ void vox_fill_kernel(const long long *__restrict__ coords, int N, int ncol, int mode, int W,
@@ -242,7 +246,7 @@ size_t sgb_voxelize_idx_workspace_bytes(int N) {
   size_t b = 0;
   b += align_up(64 * 4);
   b += align_up(cap * 8);
-  b += 4 * align_up(cap * 4);
+  b += 4 * align_up((cap + 1) * 4);
   b += 3 * align_up(((size_t)N + 1) * 4);
   b += align_up(scan_temp_elems((size_t)N + 1) * 4);
   return b + 1024;
@@ -258,9 +262,9 @@ int sgb_voxelize_idx_count(const int64_t *d_coords, int N, int ncol, int mode, i
   VoxWs w;
   SGB_REQUIRE(vox_carve(d_ws, ws_bytes, N, w), SGB_ERR_WORKSPACE, "voxelize_idx workspace too small");
   SGB_CUDA_CHECK(cudaMemsetAsync(w.keys, 0xFF, (size_t)w.cap * 8, st));
-  SGB_CUDA_CHECK(cudaMemsetAsync(w.first, 0x7F, (size_t)w.cap * 4, st));  // 0x7F7F7F7F > any index
-  SGB_CUDA_CHECK(cudaMemsetAsync(w.last, 0xFF, (size_t)w.cap * 4, st));   // -1
-  SGB_CUDA_CHECK(cudaMemsetAsync(w.cnt, 0, (size_t)w.cap * 4, st));
+  SGB_CUDA_CHECK(cudaMemsetAsync(w.first, 0x7F, ((size_t)w.cap + 1) * 4, st));  // 0x7F7F7F7F > any index
+  SGB_CUDA_CHECK(cudaMemsetAsync(w.last, 0xFF, ((size_t)w.cap + 1) * 4, st));   // -1
+  SGB_CUDA_CHECK(cudaMemsetAsync(w.cnt, 0, ((size_t)w.cap + 1) * 4, st));
   SGB_CUDA_CHECK(cudaMemsetAsync(w.scalars, 0, 64 * 4, st));
   int nb = div_up(N, 256);
   vox_insert_kernel<<<nb, 256, 0, st>>>((const long long *)d_coords, N, ncol, w);
