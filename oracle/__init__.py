@@ -40,6 +40,7 @@ def lib():
         _LIB.orc_voxelize_idx_begin.restype = ctypes.c_void_p
         _LIB.orc_bfs_cluster_begin.restype = ctypes.c_void_p
         _LIB.orc_ballquery_batch_p.restype = ctypes.c_longlong
+        _LIB.orc_ballquery_batch_p_grid.restype = ctypes.c_longlong
         _LIB.orc_octree_ball_query.restype = ctypes.c_longlong
     return _LIB
 
@@ -99,6 +100,22 @@ def ballquery_batch_p(coords, batch_idxs, batch_offsets, radius, meanActive=None
     idx = np.zeros(max(tot, 1), np.int32)
     lib().orc_ballquery_batch_p(_p(coords, _f32p), _p(batch_idxs, _i32p), _p(batch_offsets, _i32p), n,
                                 ctypes.c_float(radius), _p(idx, _i32p), ctypes.c_longlong(tot), _p(start_len, _i32p))
+    return idx[:tot], start_len
+
+
+def ballquery_batch_p_grid(coords, batch_idxs, batch_offsets, radius):
+    """ballquery_batch_p's result (same lists, same layout) from a uniform grid of cell edge ~radius: O(n * neighbours)
+    instead of O(n * segment size), for segments of hundreds of thousands of points."""
+    coords = _c(coords, np.float32)
+    batch_idxs = _c(batch_idxs, np.int32)
+    batch_offsets = _c(batch_offsets, np.int32)
+    n = coords.shape[0]
+    nb = batch_offsets.shape[0] - 1
+    start_len = np.zeros((n, 2), np.int32)
+    args = (_p(coords, _f32p), _p(batch_idxs, _i32p), _p(batch_offsets, _i32p), nb, n, ctypes.c_float(radius))
+    tot = lib().orc_ballquery_batch_p_grid(*args, None, ctypes.c_longlong(0), _p(start_len, _i32p))
+    idx = np.zeros(max(tot, 1), np.int32)
+    lib().orc_ballquery_batch_p_grid(*args, _p(idx, _i32p), ctypes.c_longlong(tot), _p(start_len, _i32p))
     return idx[:tot], start_len
 
 

@@ -178,6 +178,149 @@ long long orc_ballquery_batch_p(const float *xyz, const int32_t *batch_idxs, con
 }
 
 /* ------------------------------------------------------------------------------------------
+ * ballquery_batch_p on a uniform grid: the lists of orc_ballquery_batch_p (same test, same
+ * ascending candidate order, same first 1000) without its O(n^2) scan.
+ *
+ * Why the 27 cells hold every neighbour: all three terms of d2 are >= 0, so d2 >= fl(dx*dx)
+ * and d2 < r2 = fl(r*r) needs |fl(dx)| < |r|; rounding is monotone, so the exact |x_i - x_k|
+ * < |r| as well (likewise y, z).  The cell edge c is |r| (1 + 2^-20), or extent / 2^20 when
+ * that is larger (cell ids then fit 21 bits whatever the coordinates); the double-precision
+ * cell coordinates (x - min) / c are <= 2^20 with an error below 2^-30, so two neighbours'
+ * cells differ by at most one per axis.  A point with a NaN or Inf coordinate fails every
+ * test (d2 is NaN or Inf): it is in no cell and has no neighbour, as in the scan.
+ * Per segment b (batch_offsets[b] .. [b+1]) its finite points are sorted by (cell, index);
+ * a query merges the index-sorted runs of its 27 cells and tests candidates in ascending
+ * index until the 1000th hit.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct { int64_t key; int32_t idx; } orc_cellpt_t;
+
+static int orc_cellpt_cmp(const void *a, const void *b) {
+  const orc_cellpt_t *p = (const orc_cellpt_t *)a, *q = (const orc_cellpt_t *)b;
+  if (p->key != q->key) return p->key < q->key ? -1 : 1;
+  return (p->idx > q->idx) - (p->idx < q->idx);
+}
+
+typedef struct { orc_cellpt_t *pts; int n; double mn[3], c; } orc_grid_t;
+
+#define ORC_GRID_BITS 21
+static inline int64_t orc_cell_key(const int64_t cc[3]) {
+  return (cc[0] << (2 * ORC_GRID_BITS)) | (cc[1] << ORC_GRID_BITS) | cc[2];
+}
+
+static void orc_grid_build(orc_grid_t *g, const float *xyz, int s, int e, float radius) {
+  double mx[3] = {0, 0, 0};
+  int first = 1;
+  g->pts = (orc_cellpt_t *)malloc(sizeof(orc_cellpt_t) * (size_t)(e > s ? e - s : 1));
+  g->n = 0;
+  g->mn[0] = g->mn[1] = g->mn[2] = 0;
+  for (int k = s; k < e; k++) {
+    const float *p = xyz + 3 * (size_t)k;
+    if (!isfinite(p[0]) || !isfinite(p[1]) || !isfinite(p[2])) continue;
+    for (int a = 0; a < 3; a++) {
+      if (first || p[a] < g->mn[a]) g->mn[a] = p[a];
+      if (first || p[a] > mx[a]) mx[a] = p[a];
+    }
+    first = 0;
+  }
+  double ext = 0;
+  for (int a = 0; a < 3; a++) ext = fmax(ext, mx[a] - g->mn[a]);
+  g->c = fmax(fabs((double)radius) * (1.0 + ldexp(1.0, -20)), ext * ldexp(1.0, -20));
+  for (int k = s; k < e; k++) {
+    const float *p = xyz + 3 * (size_t)k;
+    if (!isfinite(p[0]) || !isfinite(p[1]) || !isfinite(p[2])) continue;
+    int64_t cc[3];
+    for (int a = 0; a < 3; a++) cc[a] = (int64_t)floor((p[a] - g->mn[a]) / g->c);
+    g->pts[g->n].key = orc_cell_key(cc);
+    g->pts[g->n].idx = k;
+    g->n++;
+  }
+  qsort(g->pts, (size_t)g->n, sizeof(orc_cellpt_t), orc_cellpt_cmp);
+}
+
+static int orc_grid_lower(const orc_grid_t *g, int64_t key) {
+  int lo = 0, hi = g->n;
+  while (lo < hi) {
+    int mid = lo + (hi - lo) / 2;
+    if (g->pts[mid].key < key) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+/* neighbours of xyz[i] in grid g, ascending index, first 1000; written to out (if non-NULL) */
+static int orc_grid_query(const orc_grid_t *g, const float *xyz, int i, float r2, int32_t *out) {
+  const float *o = xyz + 3 * (size_t)i;
+  if (!isfinite(o[0]) || !isfinite(o[1]) || !isfinite(o[2]) || g->n == 0) return 0;
+  const int64_t lim = (int64_t)1 << ORC_GRID_BITS;
+  double qc[3];
+  for (int a = 0; a < 3; a++) {
+    qc[a] = floor((o[a] - g->mn[a]) / g->c);
+    if (qc[a] < -1 || qc[a] > (double)lim) return 0; /* no cell of the segment within one step */
+  }
+  int lo[27], hi[27], nr = 0;
+  for (int d0 = -1; d0 <= 1; d0++)
+    for (int d1 = -1; d1 <= 1; d1++)
+      for (int d2 = -1; d2 <= 1; d2++) {
+        int64_t cc[3] = {(int64_t)qc[0] + d0, (int64_t)qc[1] + d1, (int64_t)qc[2] + d2};
+        if (cc[0] < 0 || cc[1] < 0 || cc[2] < 0 || cc[0] >= lim || cc[1] >= lim || cc[2] >= lim) continue;
+        int64_t key = orc_cell_key(cc);
+        int a = orc_grid_lower(g, key), b = orc_grid_lower(g, key + 1);
+        if (a < b) { lo[nr] = a; hi[nr] = b; nr++; }
+      }
+  /* k-way merge of the runs: a binary min-heap of runs keyed by their next index */
+  int heap[27], nh = 0;
+#define ORC_HEAD(j) (g->pts[lo[j]].idx)
+  for (int j = 0; j < nr; j++) {
+    int c = nh++;
+    while (c > 0 && ORC_HEAD(heap[(c - 1) / 2]) > ORC_HEAD(j)) { heap[c] = heap[(c - 1) / 2]; c = (c - 1) / 2; }
+    heap[c] = j;
+  }
+  int cnt = 0;
+  while (cnt < ORC_MAX_NEIGH && nh > 0) {
+    int j = heap[0];
+    int k = g->pts[lo[j]++].idx;
+    if (lo[j] == hi[j]) j = heap[--nh]; /* run exhausted: sift the last run down from the root */
+    if (nh > 0) {
+      int c = 0, v = ORC_HEAD(j);
+      for (;;) {
+        int l = 2 * c + 1, m = c, vm = v;
+        if (l < nh && ORC_HEAD(heap[l]) < vm) { m = l; vm = ORC_HEAD(heap[l]); }
+        if (l + 1 < nh && ORC_HEAD(heap[l + 1]) < vm) m = l + 1;
+        if (m == c) break;
+        heap[c] = heap[m];
+        c = m;
+      }
+      heap[c] = j;
+    }
+    if (orc_is_nb(o, xyz + 3 * (size_t)k, r2)) {
+      if (out) out[cnt] = k;
+      ++cnt;
+    }
+  }
+#undef ORC_HEAD
+  return cnt;
+}
+
+long long orc_ballquery_batch_p_grid(const float *xyz, const int32_t *batch_idxs, const int32_t *batch_offsets,
+                                     int nbatch, int n, float radius, int32_t *idx, long long idx_capacity,
+                                     int32_t *start_len) {
+  float r2 = radius * radius;
+  orc_grid_t *grids = (orc_grid_t *)calloc((size_t)(nbatch > 0 ? nbatch : 1), sizeof(orc_grid_t));
+  for (int b = 0; b < nbatch; b++) orc_grid_build(&grids[b], xyz, batch_offsets[b], batch_offsets[b + 1], radius);
+  int32_t tmp[ORC_MAX_NEIGH];
+  long long cum = 0;
+  for (int i = 0; i < n; i++) {
+    int cnt = (r2 > 0) ? orc_grid_query(&grids[batch_idxs[i]], xyz, i, r2, idx ? tmp : NULL) : 0;
+    if (idx)
+      for (int j = 0; j < cnt && cum + j < idx_capacity; j++) idx[cum + j] = tmp[j];
+    start_len[2 * (size_t)i] = (int32_t)cum; start_len[2 * (size_t)i + 1] = cnt;
+    cum += cnt;
+  }
+  for (int b = 0; b < nbatch; b++) free(grids[b].pts);
+  free(grids);
+  return cum;
+}
+
+/* ------------------------------------------------------------------------------------------
  * bfs_cluster  (bfs_cluster.cpp:33-126): find_cc :33-58, get_clusters :60-86,
  * fill_cluster_idxs_ :89-99.  Two-phase: begin() returns sumNPoint / nCluster, finish() fills.
  * ------------------------------------------------------------------------------------------ */
