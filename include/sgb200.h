@@ -311,6 +311,10 @@ long long sgb_rle_format_ids(const int32_t *h_ids, const long long *h_offs, int 
  *   sgb_bitmap_intersections: inter[r*nG+g], vert[r], void[r] from gslot int32 [N] (>= 0: gt column, -2: void, -1: other).
  *   sgb_panoptic_paste: instances visited in d_order; skipped when intersect/(size+1e-5) > skip_iou (float64), else
  *     pasted where nothing was pasted before: pan_cls[pt] = d_cls[row], pan_ids[pt] = 1, 2, ... in paste order.
+ *   sgb_bitmap_ids_count / sgb_bitmap_ids_fill: rows -> ascending point-id lists (bits >= N ignored). count: offsets
+ *     int64 [n_rows+1] (offsets[n_rows] = total), no host wait; fill, same workspace and stream: ids int32 [total].
+ *   sgb_class_bitmaps: bitmaps (zeroed here) with bit pt of row row_of_label[labels[pt]] (labels int64 [N], rows < 0 and
+ *     labels outside [0, n_labels) set nothing); counts int64 [n_rows] (may be null) = set bits per row.
  * ------------------------------------------------------------------------------------------- */
 int sgb_inst_count(const int32_t *d_proposals_idx, const float *d_mask_scores, int ms_stride, int S, int nI, float thr,
                    int32_t *d_npoint, int nP, void *stream);
@@ -329,6 +333,12 @@ int sgb_bitmap_intersections(const uint32_t *d_bitmaps, int n_rows, int N, const
                              int32_t *d_vert, int32_t *d_void, void *stream);
 int sgb_panoptic_paste(const uint32_t *d_bitmaps, int N, const int32_t *d_order, const int32_t *d_cls, int n_inst, double skip_iou,
                        uint32_t *d_prev, uint32_t *d_pan_cls, uint32_t *d_pan_ids, void *stream);
+size_t sgb_bitmap_ids_workspace_bytes(int n_rows, int N);
+int sgb_bitmap_ids_count(const uint32_t *d_bitmaps, int n_rows, int N, long long *d_offsets, void *d_ws, size_t ws_bytes,
+                         void *stream);
+int sgb_bitmap_ids_fill(const uint32_t *d_bitmaps, int n_rows, int N, int32_t *d_ids, void *d_ws, size_t ws_bytes, void *stream);
+int sgb_class_bitmaps(const int64_t *d_labels, int N, const int32_t *d_row_of_label, int n_labels, uint32_t *d_bitmaps, int n_rows,
+                      long long *d_counts, void *stream);
 
 /* Test-time transform of the reference dataloader, first step (softgroup/data/custom.py:87-107,162-164):
  * out[i, :] = xyz[i, :] @ m in float64 (xyz float32 [N,3] device, m float64 [3,3] row-major HOST, out float64 [N,3] device),

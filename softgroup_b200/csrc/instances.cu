@@ -162,6 +162,106 @@ __global__ void __launch_bounds__(kPanThreads) panoptic_paste_kernel(const uint3
   }
 }
 
+// Bitmap rows -> ascending point-id lists. A row is cut into segments of kIdSegWords words; the count pass sums the
+// popcounts of every (row, segment), a device-wide scan turns them into int64 output offsets, and the fill pass writes
+// each segment's ids at its offset. Bits at N and beyond are masked in both passes, so a row never yields an id >= N.
+constexpr int kIdThreads = 256;
+constexpr int kIdRounds = 4;
+constexpr int kIdSegWords = kIdThreads * kIdRounds;  // 1024 words = 32768 points per segment
+constexpr int kIdSegsPerCta = kIdThreads / 32;        // count pass: one warp per segment
+
+__device__ __forceinline__ uint32_t row_word(const uint32_t *__restrict__ row, long long w, int W, int N) {
+  if (w >= W) return 0u;
+  const uint32_t x = row[w];
+  const long long left = (long long)N - w * 32;  // valid bits in this word
+  return left >= 32 ? x : (left > 0 ? x & ((1u << left) - 1u) : 0u);
+}
+
+// seg_cnt[r * B + s] = set bits of segment s of row r (bits < N)
+__global__ void __launch_bounds__(kIdThreads) bitmap_ids_count_kernel(const uint32_t *__restrict__ bm, int W, int N, int B,
+                                                                      long long n_seg, long long *__restrict__ seg_cnt) {
+  const long long seg = (long long)blockIdx.x * kIdSegsPerCta + (threadIdx.x >> 5);
+  if (seg >= n_seg) return;
+  const long long r = seg / B;
+  const long long w0 = (seg - r * B) * (long long)kIdSegWords;
+  const uint32_t *row = bm + (size_t)r * W;
+  int c = 0;
+  for (int k = lane_id(); k < kIdSegWords; k += 32) c += __popc(row_word(row, w0 + k, W, N));
+  c = warp_sum(c);
+  if (lane_id() == 0) seg_cnt[seg] = c;
+}
+
+// offsets[r] = seg_off[r * B] for r <= n_rows (seg_off has n_rows * B + 1 entries, the last one the grand total)
+__global__ void bitmap_row_offsets_kernel(const long long *__restrict__ seg_off, int B, int n_rows, long long *__restrict__ offsets) {
+  const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r <= n_rows) offsets[r] = seg_off[r * B];
+}
+
+// One CTA per (row, segment): kIdRounds rounds of kIdThreads words. Per round every thread takes one word, the CTA
+// scans the popcounts (warp shuffles, then the warp totals), the ids land in shared memory at their rank and leave in
+// one coalesced copy; ids of a word come out ascending, words in order, so the segment's ids are ascending.
+__global__ void __launch_bounds__(kIdThreads) bitmap_ids_fill_kernel(const uint32_t *__restrict__ bm, int W, int N, int B,
+                                                                     const long long *__restrict__ seg_off,
+                                                                     int32_t *__restrict__ ids) {
+  __shared__ int32_t s_ids[kIdThreads * 32];
+  __shared__ int s_warp[kIdThreads / 32];
+  const long long seg = blockIdx.x;
+  long long base = seg_off[seg];
+  if (seg_off[seg + 1] == base) return;  // an empty segment is not read again
+  const long long r = seg / B;
+  const long long w0 = (seg - r * B) * (long long)kIdSegWords;
+  const uint32_t *row = bm + (size_t)r * W;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (int round = 0; round < kIdRounds; round++) {
+    const long long w = w0 + (long long)round * kIdThreads + tid;
+    uint32_t x = row_word(row, w, W, N);
+    const int c = __popc(x);
+    int inc = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int t = __shfl_up_sync(0xffffffffu, inc, o);
+      if (lane >= o) inc += t;
+    }
+    if (lane == 31) s_warp[warp] = inc;
+    __syncthreads();
+    int before = 0, round_total = 0;
+#pragma unroll
+    for (int k = 0; k < kIdThreads / 32; k++) {
+      const int t = s_warp[k];
+      before += k < warp ? t : 0;
+      round_total += t;
+    }
+    int pos = before + inc - c;
+    while (x) {
+      const int b = __ffs(x) - 1;
+      x &= x - 1;
+      s_ids[pos++] = (int32_t)(w * 32 + b);
+    }
+    __syncthreads();
+    for (int k = tid; k < round_total; k += kIdThreads) ids[base + k] = s_ids[k];
+    base += round_total;
+    __syncthreads();  // s_ids and s_warp are reused by the next round
+  }
+}
+
+// Class bitmaps: bit pt of row row_of[labels[pt]] for every point whose label has a row. A warp covers the 32 points of
+// one bitmap word, so each (row, word) has a single writer: the lanes with the same row pool their bits with one
+// match_any; counts[row] += the bits (one atomic per warp and row).
+__global__ void class_bitmaps_kernel(const int64_t *__restrict__ labels, int N, const int32_t *__restrict__ row_of, int n_labels,
+                                     uint32_t *__restrict__ bm, int W, long long *__restrict__ counts) {
+  const long long pt = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  int r = -1;
+  if (pt < N) {
+    const int64_t l = labels[pt];
+    if (l >= 0 && l < n_labels) r = __ldg(&row_of[l]);
+  }
+  const unsigned peers = __match_any_sync(0xffffffffu, r);
+  if (r >= 0 && lane_id() == __ffs(peers) - 1) {
+    bm[(size_t)r * W + (pt >> 5)] = peers;
+    if (counts) atomicAdd((unsigned long long *)&counts[r], (unsigned long long)__popc(peers));
+  }
+}
+
 }  // namespace sgb
 
 using namespace sgb;
@@ -310,6 +410,75 @@ int sgb_panoptic_paste(const uint32_t *d_bitmaps, int N, const int32_t *d_order,
   const int W = (int)sgb_bitmap_words(N);
   SGB_CUDA_CHECK(cudaMemsetAsync(d_prev, 0, (size_t)W * 4, st));
   panoptic_paste_kernel<<<1, kPanThreads, 0, st>>>(d_bitmaps, W, N, d_order, d_cls, n_inst, skip_iou, d_prev, d_pan_cls, d_pan_ids);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+static long long id_segments(int n_rows, int N) {
+  return (long long)std::max(n_rows, 0) * div_up((long long)sgb_bitmap_words(N), kIdSegWords);
+}
+
+size_t sgb_bitmap_ids_workspace_bytes(int n_rows, int N) {
+  const size_t n = (size_t)id_segments(n_rows, N) + 1;
+  return align_up(n * 8) + align_up(scan_temp_elems(n) * 8) + 1024;
+}
+
+// Count pass: d_offsets int64 [n_rows + 1] = exclusive prefix of the rows' set bits (bits < N); d_offsets[n_rows] is the
+// total. No host wait. The per-segment offsets stay in the workspace for sgb_bitmap_ids_fill.
+int sgb_bitmap_ids_count(const uint32_t *d_bitmaps, int n_rows, int N, long long *d_offsets, void *d_ws, size_t ws_bytes,
+                         void *stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SGB_REQUIRE(n_rows >= 0 && N >= 0 && d_offsets, SGB_ERR_ARG, "bitmap_ids_count arguments");
+  if (n_rows == 0) { SGB_CUDA_CHECK(cudaMemsetAsync(d_offsets, 0, 8, st)); return SGB_OK; }
+  const int W = (int)sgb_bitmap_words(N);
+  const int B = div_up(W, kIdSegWords);
+  const long long n_seg = id_segments(n_rows, N);
+  SGB_REQUIRE(n_seg < (1ll << 31), SGB_ERR_RANGE, "bitmap_ids: rows * segments must stay below 2^31");
+  Arena a(d_ws, ws_bytes);
+  long long *seg = a.take<long long>((size_t)n_seg + 1);
+  long long *tmp = a.take<long long>(scan_temp_elems((size_t)n_seg + 1));
+  SGB_REQUIRE(d_bitmaps && seg && tmp, SGB_ERR_WORKSPACE, "bitmap_ids workspace too small");
+  bitmap_ids_count_kernel<<<div_up(n_seg, kIdSegsPerCta), kIdThreads, 0, st>>>(d_bitmaps, W, N, B, n_seg, seg);
+  SGB_LAUNCH_CHECK();
+  const int rc = exclusive_scan_i64(seg, seg, (size_t)n_seg, seg + n_seg, tmp, st);
+  if (rc) return rc;
+  bitmap_row_offsets_kernel<<<div_up((long long)n_rows + 1, 256), 256, 0, st>>>(seg, B, n_rows, d_offsets);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+// Fill pass, after sgb_bitmap_ids_count on the same workspace and stream: d_ids int32 [total], the ids of row r
+// ascending at [offsets[r], offsets[r + 1]).
+int sgb_bitmap_ids_fill(const uint32_t *d_bitmaps, int n_rows, int N, int32_t *d_ids, void *d_ws, size_t ws_bytes, void *stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SGB_REQUIRE(n_rows >= 0 && N >= 0, SGB_ERR_ARG, "bitmap_ids_fill arguments");
+  if (n_rows == 0) return SGB_OK;
+  const int W = (int)sgb_bitmap_words(N);
+  const int B = div_up(W, kIdSegWords);
+  const long long n_seg = id_segments(n_rows, N);
+  SGB_REQUIRE(n_seg < (1ll << 31), SGB_ERR_RANGE, "bitmap_ids: rows * segments must stay below 2^31");
+  Arena a(d_ws, ws_bytes);
+  const long long *seg = a.take<long long>((size_t)n_seg + 1);
+  SGB_REQUIRE(d_bitmaps && d_ids && seg, SGB_ERR_WORKSPACE, "bitmap_ids workspace too small");
+  bitmap_ids_fill_kernel<<<(unsigned)n_seg, kIdThreads, 0, st>>>(d_bitmaps, W, N, B, seg, d_ids);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+// Class bitmaps (zeroed here): d_bitmaps uint32 [n_rows][W]; row d_row_of_label[l] (or -1) for label l in [0, n_labels);
+// labels outside that range set no bit. d_counts int64 [n_rows] (may be null) receives the rows' set bits.
+int sgb_class_bitmaps(const int64_t *d_labels, int N, const int32_t *d_row_of_label, int n_labels, uint32_t *d_bitmaps, int n_rows,
+                      long long *d_counts, void *stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SGB_REQUIRE(N >= 0 && n_labels >= 0 && n_rows >= 0, SGB_ERR_ARG, "class_bitmaps arguments");
+  if (n_rows == 0) return SGB_OK;
+  SGB_REQUIRE(d_bitmaps, SGB_ERR_ARG, "null bitmaps");
+  const int W = (int)sgb_bitmap_words(N);
+  SGB_CUDA_CHECK(cudaMemsetAsync(d_bitmaps, 0, (size_t)n_rows * W * 4, st));
+  if (d_counts) SGB_CUDA_CHECK(cudaMemsetAsync(d_counts, 0, (size_t)n_rows * 8, st));
+  if (N == 0 || n_labels == 0) return SGB_OK;
+  SGB_REQUIRE(d_labels && d_row_of_label, SGB_ERR_ARG, "class_bitmaps pointers");
+  class_bitmaps_kernel<<<div_up(N, 256), 256, 0, st>>>(d_labels, N, d_row_of_label, n_labels, d_bitmaps, W, d_counts);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

@@ -45,14 +45,16 @@ def pointwise_injection(scan, sigma=0.03, seed=0, logit=8.0, fragments=1, confus
     return torch.from_numpy(scores).cuda(), torch.from_numpy(off).cuda()
 
 
-def run_scan(model, host_batch, device_only=False, inject_pointwise=None):
+def run_scan(model, host_batch, device_only=False, inject_pointwise=None, device_results=False):
     """End-to-end call a user makes: pinned host tensors in, result dict out. Point->voxel hashing runs on the GPU
-    (voxelization_idx with CUDA tensors), then SoftGroup.forward_test."""
+    (voxelization_idx with CUDA tensors), then SoftGroup.forward_test. device_results: the results stay CUDA tensors on
+    the current stream (forward_test's device_results form)."""
     dev = {k: (v.cuda(non_blocking=True) if isinstance(v, torch.Tensor) else v) for k, v in host_batch.items()}
     voxel_coords, v2p_map, p2v_map = ops.voxelization_idx(dev['coords'], dev['batch_size'])
     dev.update(voxel_coords=voxel_coords, v2p_map=v2p_map, p2v_map=p2v_map)
     dev.pop('coords')
-    return model.forward_test(device_only=device_only, inject_pointwise=inject_pointwise, host_inputs=host_batch, **dev)
+    return model.forward_test(device_only=device_only, device_results=device_results, inject_pointwise=inject_pointwise,
+                              host_inputs=host_batch, **dev)
 
 
 class ScanPipeline(object):
@@ -108,11 +110,13 @@ class ScanPipeline(object):
         out = [f.result() for f in futs]
         return [o[0] for o in out], [o[1] for o in out]
 
-    def run_scans(self, host_batches, inject_pointwise=None, device_only=False):
-        """The end-to-end call for a sequence of scans: pinned host batches in, result dicts out (input order)."""
+    def run_scans(self, host_batches, inject_pointwise=None, device_only=False, device_results=False):
+        """The end-to-end call for a sequence of scans: pinned host batches in, result dicts out (input order). With
+        device_results the dicts hold CUDA tensors written on the workers' streams; they are complete when this returns."""
         inj = inject_pointwise if isinstance(inject_pointwise, (list, tuple)) and inject_pointwise and \
             isinstance(inject_pointwise[0], (list, tuple)) else [inject_pointwise] * len(host_batches)
-        res, evs = self.map(lambda a: run_scan(self.model, a[0], device_only=device_only, inject_pointwise=a[1]),
+        res, evs = self.map(lambda a: run_scan(self.model, a[0], device_only=device_only, inject_pointwise=a[1],
+                                               device_results=device_results),
                             list(zip(host_batches, inj)))
         for e in evs:
             e.synchronize()

@@ -219,6 +219,11 @@ class SoftGroup(nn.Module):
         self._events = []
         self._mark('start')
         device_only = kwargs.get('device_only', False)  # bench: keep results on the GPU (no numpy / RLE)
+        # the scan's results as CUDA tensors: point-wise predictions, instances as point-id lists, panoptic labels
+        device_results = kwargs.get('device_results', False)
+        if device_only and device_results:
+            raise ValueError('forward_test: device_only and device_results are two different result forms; pass one')
+        host_results = not (device_only or device_results)
         # The reference returns the caller's own inputs (labels, coords_float, feats) as numpy arrays, reading them back from
         # the GPU (softgroup.py:317-331). When the caller still holds them on the host (harness.run_scan), `host_inputs`
         # hands those tensors over and the result dict carries views of them: 7.8 of the 12.3 MB read back per 150k-point
@@ -262,7 +267,7 @@ class SoftGroup(nn.Module):
         ret = dict(scan_id=scan_ids[0] if scan_ids else None)
         # the reference reads these back with blocking .cpu() calls in the middle of the forward (softgroup.py:317-331);
         # here the copies go to pinned memory on a side stream and are awaited once, after the instance branch
-        fetch = _HostFetcher(semantic_scores.device) if not device_only else None
+        fetch = _HostFetcher(semantic_scores.device) if host_results else None
 
         def passthrough(name, dev_tensor, host_key):
             h = host_inputs.get(host_key) if (host_inputs is not None and not x4_split) else None
@@ -271,7 +276,7 @@ class SoftGroup(nn.Module):
             else:
                 fetch.add(name, dev_tensor)
 
-        if not device_only:
+        if host_results:
             if 'semantic' in eval_tasks or 'panoptic' in eval_tasks:
                 passthrough('semantic_labels', semantic_labels, 'semantic_labels')
                 passthrough('instance_labels', instance_labels, 'instance_labels')
@@ -297,10 +302,16 @@ class SoftGroup(nn.Module):
             self._mark('instance_head')
             inst = self.get_instances(scan_ids[0] if scan_ids else None, proposals_idx, semantic_scores, cls_scores,
                                       iou_scores, mask_scores, v2p_map=v2p_map, lvl_fusion=lvl_fusion,
-                                      device_only=device_only)
+                                      device_only=device_only, device_results=device_results)
             self._mark('get_instances')
             if device_only:
                 ret.update(device_instances=inst, proposals_idx=proposals_idx, proposals_offset=proposals_offset)
+            elif device_results:
+                ret.update(instances=inst)
+                if 'panoptic' in eval_tasks:
+                    bm, npts = self._tls.instance_bitmaps
+                    ret.update(panoptic_preds=self.panoptic_fusion_device(
+                        semantic_preds[v2p_map.long()] if lvl_fusion else semantic_preds, inst, bm, npts))
             else:
                 if 'instance' in eval_tasks:
                     ret.update(dict(pred_instances=inst))
@@ -315,12 +326,15 @@ class SoftGroup(nn.Module):
                     ret.update(panoptic_preds=pan)
         if device_only:
             ret.update(semantic_preds=semantic_preds, pt_offsets=pt_offsets)
+        elif device_results:  # per point, as get_point_wise_results returns them (softgroup.py:524-536)
+            ret.update(semantic_preds=semantic_preds[v2p_map.long()] if lvl_fusion else semantic_preds,
+                       offset_preds=pt_offsets[v2p_map.long()] if lvl_fusion else pt_offsets)
         else:
             ret.update(fetch.finish())
-        if semantic_scores.is_cuda and not device_only:
+        if semantic_scores.is_cuda and host_results:
             # an activation beyond the fp16 hi/lo range raises here instead of saturating silently (the host has just waited
-            # for the results anyway). device_only callers keep the forward free of host waits and call
-            # spconv.check_overflow() themselves where they synchronise.
+            # for the results anyway). device_only / device_results callers keep the forward free of this host wait and
+            # call spconv.check_overflow() themselves where they synchronise.
             spconv.check_overflow()
         if self.profile_stages:
             torch.cuda.synchronize()
@@ -686,13 +700,17 @@ class SoftGroup(nn.Module):
     # ------------------------------------------------------------------------------------------------------
     @force_fp32(apply_to=('semantic_scores', 'cls_scores', 'iou_scores', 'mask_scores'))
     def get_instances(self, scan_id, proposals_idx, semantic_scores, cls_scores, iou_scores, mask_scores,
-                      v2p_map=None, lvl_fusion=False, device_only=False):
+                      v2p_map=None, lvl_fusion=False, device_only=False, device_results=False):
         """softgroup.py:537-604 without dense masks.
 
         For every instance class i and proposal p (class-major, proposal order -- the order in which the reference
         concatenates its lists): kept iff cls_score[p,i] > cls_score_thr and
-        #{points of p with mask_score[:, i] > mask_score_thr} >= min_npoint."""
+        #{points of p with mask_score[:, i] > mask_score_thr} >= min_npoint.
+        device_results: the same instances as CUDA tensors, dict(label_id int32 [n], conf f32 [n], point_offsets int64
+        [n + 1], point_ids int32 [total]) -- instance k's points, ascending, are point_ids[point_offsets[k]:point_offsets[k + 1]]."""
         if proposals_idx.size(0) == 0:
+            if device_results:
+                return self._no_device_instances(semantic_scores.device, v2p_map.numel() if lvl_fusion else semantic_scores.size(0))
             return []
         semantic_pred_rows = None
         if lvl_fusion:
@@ -718,6 +736,15 @@ class SoftGroup(nn.Module):
             keep[:, i] = False
         if device_only:
             return dict(keep=keep, score=score, npoint=npoint)
+        if device_results:
+            sem_pts = None
+            if self.sem2ins_classes:
+                sem_pts = semantic_pred_rows if lvl_fusion else semantic_scores.max(1)[1]
+            bm, label_id, conf, total = self._instance_bitmaps_in_order(proposals_idx.contiguous(), mask_scores, mask_thr,
+                                                                       keep, score, npoint, sem_pts, num_points)
+            self._tls.instance_bitmaps = (bm, num_points)  # reused by panoptic_fusion_device in the same forward (same thread)
+            point_offsets, point_ids = inst_ops.bitmap_point_ids(bm, num_points, total=total)
+            return dict(label_id=label_id, conf=conf, point_offsets=point_offsets, point_ids=point_ids)
         # kept (class, proposal) pairs in the reference's order (class-major, proposal order) -> one bitmap each; run
         # boundaries are found on the GPU and only (start, end) pairs are read back (rle.py:5-19 on the host before)
         bitmaps, kc, kp = inst_ops.instance_bitmaps(proposals_idx.contiguous(), mask_scores, nI, mask_thr, keep, num_points)
@@ -745,6 +772,68 @@ class SoftGroup(nn.Module):
                 instances.append(dict(scan_id=scan_id, label_id=i + 1, conf=conf_np[k], pred_mask=rles[k]))
                 k += 1
         return instances
+
+    def _no_device_instances(self, dev, num_points):
+        self._tls.instance_bitmaps = (torch.zeros((0, inst_ops.bitmap_words(num_points)), dtype=torch.int32, device=dev),
+                                      num_points)
+        return dict(label_id=torch.zeros(0, dtype=torch.int32, device=dev), conf=torch.zeros(0, dtype=torch.float32, device=dev),
+                    point_offsets=torch.zeros(1, dtype=torch.int64, device=dev),
+                    point_ids=torch.zeros(0, dtype=torch.int32, device=dev))
+
+    def _instance_bitmaps_in_order(self, proposals_idx, mask_scores, mask_thr, keep, score, npoint, sem_pts, num_points):
+        """Bitmaps of every instance get_instances returns, in its order: class-major, the kept proposals of a class in
+        proposal order, a sem2ins class as one instance (its points: semantic prediction == class, conf 1.0) at its
+        class's position. One host read: the instance count and the point total together (sizes of the bitmaps and of the
+        point-id list). A proposal holds a point at most once, so its bitmap row has npoint[p, i] bits.
+        Returns (bitmaps int32 [n, W], label_id int32 [n], conf f32 [n], total points)."""
+        dev = keep.device
+        nP, nI = keep.shape
+        # (class, proposal) cells class-major, plus a last column per class for its sem2ins instance: instance k is the
+        # k-th true cell
+        cells = torch.zeros((nI, nP + 1), dtype=torch.bool, device=dev)
+        cells[:, :nP] = keep.t()
+        size = torch.zeros((nI, nP + 1), dtype=torch.int64, device=dev)
+        size[:, :nP] = npoint.t()
+        conf = torch.ones((nI, nP + 1), dtype=torch.float32, device=dev)
+        conf[:, :nP] = score.t()
+        sem2ins = [i for i in range(nI) if i in self.sem2ins_classes]
+        if sem2ins:
+            cls_bm, cls_cnt = inst_ops.class_bitmaps(sem_pts.contiguous(), sem2ins, num_points)
+            rows = inst_ops.to_device_async(np.asarray(sem2ins), torch.int64, dev)
+            cells[:, nP] = inst_ops.to_device_async(np.isin(np.arange(nI), sem2ins), torch.bool, dev)
+            size[:, nP] = torch.zeros(nI, dtype=torch.int64, device=dev).index_copy_(0, rows, cls_cnt)
+        flat = cells.view(-1)
+        slot = torch.cumsum(flat, 0) - 1
+        n_inst, total = (int(v) for v in torch.stack([flat.sum(), torch.where(flat, size.view(-1), 0).sum()]).cpu())
+        slot = torch.where(flat, slot, torch.full_like(slot, -1)).view(nI, nP + 1)
+        bm = inst_ops.scatter_instance_bitmaps(proposals_idx, mask_scores, nI, mask_thr, slot[:, :nP].int().contiguous(),
+                                               n_inst, num_points)
+        if sem2ins and n_inst:
+            bm.index_copy_(0, slot[:, nP].index_select(0, rows), cls_bm)
+        dst = torch.where(flat, slot.view(-1), n_inst)  # cells that are no instance land in a spare last entry
+        label_id = torch.empty(n_inst + 1, dtype=torch.int32, device=dev)
+        label_id.scatter_(0, dst, torch.arange(1, nI + 1, dtype=torch.int32, device=dev).repeat_interleave(nP + 1))
+        conf_out = torch.empty(n_inst + 1, dtype=torch.float32, device=dev)
+        conf_out.scatter_(0, dst, conf.view(-1))
+        return bm, label_id[:n_inst], conf_out[:n_inst], total
+
+    def panoptic_fusion_device(self, semantic_preds, instances, bitmaps, num_points):
+        """panoptic_fusion on the device results: semantic_preds int64 [N] per point, `instances` get_instances'
+        device_results dict, bitmaps row k the mask of its instance k. The visiting order is numpy's argsort of the
+        confidences (one host read); returns int64 [N] CUDA holding the uint32 values panoptic_fusion returns."""
+        dev = semantic_preds.device
+        n_inst = bitmaps.size(0)
+        order = torch.zeros(0, dtype=torch.int32, device=dev)
+        if n_inst:
+            scores = instances['conf'].cpu().numpy()
+            order = inst_ops.to_device_async(np.argsort(scores)[::-1].astype(np.int32), torch.int32, dev)
+        cls_offset = self.semantic_classes - self.instance_classes - 1
+        pan_cls, pan_ids = inst_ops.panoptic_paste(bitmaps, order, instances['label_id'] + cls_offset, semantic_preds,
+                                                   float(self._cfg(self.test_cfg, 'panoptic_skip_iou')), num_points)
+        pan_cls, pan_ids = pan_cls.long() & 0xFFFFFFFF, pan_ids.long()
+        ignore = (pan_cls >= 11) & (pan_ids == 0)
+        preds = ((pan_cls & 0xFFFF) | (pan_ids << 16)) & 0xFFFFFFFF
+        return torch.where(ignore, torch.full_like(preds, self.semantic_classes), preds)
 
     def panoptic_fusion_gpu(self, semantic_preds, instance_preds, bitmaps, num_points):
         """softgroup.py:606-639 on the GPU: `bitmaps` row k is the mask of instance_preds[k]. The visiting order is the

@@ -79,6 +79,10 @@ SIGNATURES = {
     'sgb_rle_format_runs': (c_longlong, [_P, _P, c_int, _P, c_longlong, _P]),
     'sgb_bitmap_intersections': (c_int, [_P, c_int, c_int, _P, c_int, _P, _P, _P, _P]),
     'sgb_panoptic_paste': (c_int, [_P, c_int, _P, _P, c_int, c_double, _P, _P, _P, _P]),
+    'sgb_bitmap_ids_workspace_bytes': (c_size_t, [c_int, c_int]),
+    'sgb_bitmap_ids_count': (c_int, [_P, c_int, c_int, _P, _P, c_size_t, _P]),
+    'sgb_bitmap_ids_fill': (c_int, [_P, c_int, c_int, _P, _P, c_size_t, _P]),
+    'sgb_class_bitmaps': (c_int, [_P, c_int, _P, c_int, _P, c_int, _P, _P]),
     'sgb_affine3_f64': (c_int, [_P, _P, _P, c_int, _P]),
     'sgb_rle_format_ids': (c_longlong, [_P, _P, c_int, _P, c_longlong, _P]),
 }

@@ -47,6 +47,18 @@ def instance_bitmaps(proposals_idx, mask_scores, n_classes, thr, keep, n_points)
     return bm, kc, kp
 
 
+def scatter_instance_bitmaps(proposals_idx, mask_scores, n_classes, thr, slot, n_rows, n_points):
+    """slot int32 [nI, nP] (class-major: bitmap row of (class i, proposal p), or -1) -> bitmaps int32 [n_rows, W], zeroed,
+    with the mask of every slotted pair set (rows without a pair stay zero). No host wait."""
+    assert slot.dtype == torch.int32 and slot.is_contiguous() and slot.size(0) == n_classes
+    bm = torch.empty((n_rows, bitmap_words(n_points)), dtype=torch.int32, device=proposals_idx.device)
+    with profiler.record('inst_scatter', 8 * proposals_idx.size(0) + 4 * bm.numel()):
+        check(_lib.lib().sgb_inst_scatter(ptr(proposals_idx), ptr(mask_scores), mask_scores.stride(0), proposals_idx.size(0),
+                                          n_classes, slot.size(1), float(thr), ptr(slot), ptr(bm), n_rows, int(n_points),
+                                          _stream()), 'sgb_inst_scatter')
+    return bm
+
+
 def bitmaps_from_pairs(rows, points, n_rows, n_points):
     """(row, point) int32 pairs -> bitmaps int32 [n_rows, W] (rows < 0 are skipped)."""
     assert rows.is_cuda and rows.dtype == torch.int32 and points.dtype == torch.int32
@@ -109,6 +121,55 @@ def bitmap_intersections(bitmaps, gslot, n_gt, n_points):
     check(_lib.lib().sgb_bitmap_intersections(ptr(bitmaps), n_rows, int(n_points), ptr(gslot.contiguous()), int(n_gt), ptr(inter),
                                               ptr(vert), ptr(void), _stream()), 'sgb_bitmap_intersections')
     return inter[:, :n_gt], vert, void
+
+
+def to_device_async(a, dtype, device):
+    """Small host array -> CUDA tensor without a host wait: staged in pinned memory, copied on the current stream (torch's
+    caching host allocator keeps the pinned block until the copy has run)."""
+    h = torch.from_numpy(np.ascontiguousarray(a)).to(dtype).pin_memory()
+    return h.to(device, non_blocking=True)
+
+
+def bitmap_point_ids(bitmaps, n_points, total=None):
+    """bitmaps int32 [n_rows, W] (CUDA) -> (offsets int64 [n_rows + 1], ids int32 [total]): the ids of row r, ascending, are
+    ids[offsets[r]:offsets[r + 1]]; bits at n_points and beyond are ignored. `total` sizes `ids` when the caller knows the
+    number of set bits; otherwise it is read back (one host wait between the count and the fill pass)."""
+    assert bitmaps.is_cuda and bitmaps.dtype == torch.int32 and bitmaps.is_contiguous()
+    n_rows = bitmaps.size(0)
+    assert bitmaps.size(1) == bitmap_words(n_points) or n_rows == 0
+    L = _lib.lib()
+    dev = bitmaps.device
+    offsets = torch.empty(n_rows + 1, dtype=torch.int64, device=dev)
+    ws = _ws(L.sgb_bitmap_ids_workspace_bytes(n_rows, int(n_points)), dev)
+    with profiler.record('bitmap_ids_count', 4 * bitmaps.numel()):
+        check(L.sgb_bitmap_ids_count(ptr(bitmaps), n_rows, int(n_points), ptr(offsets), ptr(ws), ws.numel(), _stream()),
+              'sgb_bitmap_ids_count')
+    if total is None:
+        total = int(offsets[-1].item())
+    ids = torch.empty(max(int(total), 1), dtype=torch.int32, device=dev)
+    with profiler.record('bitmap_ids_fill', 4 * bitmaps.numel() + 4 * int(total)):
+        check(L.sgb_bitmap_ids_fill(ptr(bitmaps), n_rows, int(n_points), ptr(ids), ptr(ws), ws.numel(), _stream()),
+              'sgb_bitmap_ids_fill')
+    return offsets, ids[:int(total)]
+
+
+def class_bitmaps(labels, classes, n_points):
+    """labels int64 [N] (CUDA), classes: distinct non-negative ints (host) -> (bitmaps int32 [len(classes), W] with row k
+    marking the points labelled classes[k], counts int64 [len(classes)] of their set bits). No host wait."""
+    assert labels.is_cuda and labels.dtype == torch.int64 and labels.is_contiguous() and labels.numel() == int(n_points)
+    classes = [int(c) for c in classes]
+    assert len(set(classes)) == len(classes) and all(c >= 0 for c in classes)
+    dev = labels.device
+    n_rows = len(classes)
+    row_of = np.full(max(classes) + 1 if classes else 0, -1, np.int32)
+    row_of[classes] = np.arange(n_rows, dtype=np.int32)
+    row_of_d = to_device_async(row_of, torch.int32, dev)
+    bm = torch.empty((n_rows, bitmap_words(n_points)), dtype=torch.int32, device=dev)
+    counts = torch.empty(n_rows, dtype=torch.int64, device=dev)
+    with profiler.record('class_bitmaps', 8 * int(n_points) + 4 * bm.numel()):
+        check(_lib.lib().sgb_class_bitmaps(ptr(labels), int(n_points), ptr(row_of_d), row_of.size, ptr(bm), n_rows, ptr(counts),
+                                           _stream()), 'sgb_class_bitmaps')
+    return bm, counts
 
 
 def panoptic_paste(bitmaps, order, cls_values, semantic_preds, skip_iou, n_points):
