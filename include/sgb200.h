@@ -340,6 +340,38 @@ int sgb_bitmap_ids_fill(const uint32_t *d_bitmaps, int n_rows, int N, int32_t *d
 int sgb_class_bitmaps(const int64_t *d_labels, int N, const int32_t *d_row_of_label, int n_labels, uint32_t *d_bitmaps, int n_rows,
                       long long *d_counts, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Point-id lists (the instances of forward_test(device_results=True)): list k is d_ids[d_offsets[k] .. d_offsets[k+1]),
+ * d_offsets int64 [n+1] non-decreasing with d_offsets[0] = 0 and d_offsets[n] = total, d_ids int32 [total], ids in [0, N).
+ * n may be any int, total any int64 (beyond 2^31 included). Ids outside [0, N) are never dereferenced: they count for no
+ * op and in no count. Both calls enqueue on `stream` and never wait for the host; the id space is cut into fixed
+ * 256-id chunks, so one long list or many short ones spread over the whole GPU alike.
+ *   sgb_id_lists_reduce: per list and channel, over the rows d_values[id * ld + c] (f32 [N, C], row stride ld >= C, any
+ *     C >= 1) of its ids, the ops in `ops` (SGB_REDUCE_* mask): d_min / d_max / d_mean f32 [n, C] (NULL when not asked
+ *     for), and d_counts int64 [n] (always) = ids in [0, N) per list.
+ *     min / max are exact, with the semantics of sgb_sec_min / sgb_sec_max: NaN never wins, an empty list gives +inf /
+ *     -inf, only the sign of a zero result is unspecified.
+ *     mean: float64 partial sums over each 256-id chunk, combined in chunk order (no float atomics), so the same bits on
+ *     every run; an empty list gives NaN. Not order-exact: per element, with len the count and mean64 the float64 mean,
+ *     |out - mean64| <= 2^-24 * |mean64| + (len/256 + 300) * 2^-52 * sum|x| / len.
+ *     Launches: 2 (1 when total = 0; none when n = 0). Workspace: sgb_id_lists_reduce_workspace_bytes(total, C).
+ *   sgb_id_lists_point_map: d_map int32 [N]: map[p] = the k of the highest d_conf[k] (f32 [n]) among the lists holding p;
+ *     ties go to the smaller k, -0.0 ties with +0.0, a NaN confidence ranks below every number (-inf included), and a
+ *     point in no list gets -1. One pass does a 64-bit atomicMax of (ordered bits of conf, ~k) per id into a per-point
+ *     key, a second decodes it: the result does not depend on execution order. Launches: 2 (1 when n or total is 0), after
+ *     one memset. Workspace: sgb_id_lists_point_map_workspace_bytes(N).
+ * ------------------------------------------------------------------------------------------- */
+#define SGB_REDUCE_MIN 1
+#define SGB_REDUCE_MAX 2
+#define SGB_REDUCE_MEAN 4
+size_t sgb_id_lists_reduce_workspace_bytes(long long total, int C);
+int sgb_id_lists_reduce(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_values,
+                        long long ld, int C, int ops, float *d_min, float *d_max, float *d_mean, long long *d_counts, void *d_ws,
+                        size_t ws_bytes, void *stream);
+size_t sgb_id_lists_point_map_workspace_bytes(int N);
+int sgb_id_lists_point_map(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_conf,
+                           int32_t *d_map, void *d_ws, size_t ws_bytes, void *stream);
+
 /* Test-time transform of the reference dataloader, first step (softgroup/data/custom.py:87-107,162-164):
  * out[i, :] = xyz[i, :] @ m in float64 (xyz float32 [N,3] device, m float64 [3,3] row-major HOST, out float64 [N,3] device),
  * accumulated like the BLAS kernels numpy calls: fma(z, m2j, fma(y, m1j, x * m0j)). */

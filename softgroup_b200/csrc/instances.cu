@@ -262,6 +262,194 @@ __global__ void class_bitmaps_kernel(const int64_t *__restrict__ labels, int N, 
   }
 }
 
+// ---- per-list reductions and the point map over int64-offset id lists ----------------------------------------------
+// The id space [0, total) is cut into chunks of kListChunk ids, one warp per chunk, so the work per warp is the same
+// whatever the list lengths. A list inside one chunk is finished by that warp. A list that crosses a chunk boundary
+// leaves one partial per chunk it touches: in the chunk where it starts, the "tail" slot (2c + 1); in every later chunk,
+// the "head" slot (2c). Those lists are finished by id_reduce_lists_kernel, which combines the partials in chunk order.
+// Sums are float64 and every combination order is fixed, so a mean has the same bits on every run.
+constexpr int kListThreads = 256;
+constexpr int kListWarps = kListThreads / 32;
+constexpr int kListChunk = 256;
+constexpr int kListCtasPerSm = 6;  // 40 registers, no spills (ptxas -v): 48 of 64 warps per multiprocessor
+
+__device__ __forceinline__ int pow2_lanes(int C) {  // channel lanes: pow2 >= min(C, 32)
+  int cw = 1;
+  while (cw < C && cw < 32) cw <<= 1;
+  return cw;
+}
+
+// last k in [0, n) with off[k] <= i (0 if none)
+__device__ __forceinline__ int list_of(const long long *__restrict__ off, int n, long long i) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (off[mid] <= i) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+__global__ void __launch_bounds__(kListThreads, kListCtasPerSm) id_reduce_chunks_kernel(
+    const long long *__restrict__ off, int n, const int32_t *__restrict__ ids, long long total, int N,
+    const float *__restrict__ vals, long long ld, int C, int ops, float *__restrict__ omin, float *__restrict__ omax,
+    float *__restrict__ omean, long long *__restrict__ ocnt, double *__restrict__ psum, float *__restrict__ pmin,
+    float *__restrict__ pmax, int32_t *__restrict__ pcnt) {
+  const int lane = lane_id(), Cw = pow2_lanes(C), rows = 32 / Cw;
+  const int tx = lane % Cw, ty = lane / Cw;
+  const long long nch = (total + kListChunk - 1) / kListChunk;
+  for (long long ch = (long long)blockIdx.x * kListWarps + (threadIdx.x >> 5); ch < nch; ch += (long long)gridDim.x * kListWarps) {
+    const long long cs = ch * kListChunk, ce = min(cs + kListChunk, total);
+    int k = list_of(off, n, cs);
+    long long r0 = cs;
+    while (r0 < ce) {
+      while (k < n - 1 && off[k + 1] <= r0) k++;  // empty lists have no ids
+      const long long start = off[k], end = min(off[k + 1], total);
+      const long long e = min(end, ce);
+      r0 = max(r0, start);  // ids below offsets[0] belong to no list
+      if (e <= r0) break;   // nor do ids at offsets[n] and beyond
+      const bool whole = start >= cs && end <= ce;
+      const long long slot = 2 * ch + (start < cs ? 0 : 1);
+      for (int c0 = 0; c0 < C; c0 += Cw) {
+        const int c = c0 + tx;
+        double sum = 0.0;
+        float mn = INFINITY, mx = -INFINITY;
+        int cnt = 0;
+        for (long long i = r0 + ty; i < e; i += rows) {
+          const int id = __ldg(&ids[i]);
+          if ((unsigned)id >= (unsigned)N) continue;  // outside [0, N): never read
+          cnt++;
+          if (c < C) {
+            const float x = __ldg(&vals[(size_t)id * ld + c]);
+            mn = (x < mn) ? x : mn;  // the comparisons of seg_minmax_kernel: NaN never wins
+            mx = (x > mx) ? x : mx;
+            sum += (double)x;
+          }
+        }
+        for (int o = Cw; o < 32; o <<= 1) {  // across the row lanes; lane ty == 0 holds a fixed-order result
+          sum += __shfl_xor_sync(0xffffffffu, sum, o);
+          const float a = __shfl_xor_sync(0xffffffffu, mn, o), b = __shfl_xor_sync(0xffffffffu, mx, o);
+          mn = (a < mn) ? a : mn;
+          mx = (b > mx) ? b : mx;
+          cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        }
+        if (ty == 0 && c < C) {
+          if (whole) {
+            const size_t o = (size_t)k * C + c;
+            if (ops & SGB_REDUCE_MIN) omin[o] = mn;
+            if (ops & SGB_REDUCE_MAX) omax[o] = mx;
+            if (ops & SGB_REDUCE_MEAN) omean[o] = (float)(sum / (double)cnt);  // 0 / 0 = NaN for no id in [0, N)
+            if (c == 0) ocnt[k] = cnt;
+          } else {
+            const size_t o = (size_t)slot * C + c;
+            psum[o] = sum;
+            pmin[o] = mn;
+            pmax[o] = mx;
+            if (c == 0) pcnt[slot] = cnt;
+          }
+        }
+      }
+      r0 = e;
+    }
+  }
+}
+
+// Lists the chunk pass did not finish: empty ones, and those spanning chunks (partials tail[c0], head[c0 + 1 .. c1]).
+// One CTA per list; per channel, a thread sums every rows_par-th partial in order, then a fixed shared-memory tree.
+__global__ void __launch_bounds__(kListThreads) id_reduce_lists_kernel(
+    const long long *__restrict__ off, int n, long long total, int C, int ops, const double *__restrict__ psum,
+    const float *__restrict__ pmin, const float *__restrict__ pmax, const int32_t *__restrict__ pcnt,
+    float *__restrict__ omin, float *__restrict__ omax, float *__restrict__ omean, long long *__restrict__ ocnt) {
+  __shared__ double s_sum[kListThreads];
+  __shared__ float s_min[kListThreads], s_max[kListThreads];
+  __shared__ long long s_cnt[kListWarps];
+  const int Cw = pow2_lanes(C), rows_par = kListThreads / Cw;
+  const int tx = threadIdx.x % Cw, ty = threadIdx.x / Cw;
+  for (int k = blockIdx.x; k < n; k += gridDim.x) {
+    const long long s = min(off[k], total), e = min(off[k + 1], total);
+    const long long c0 = s / kListChunk, c1 = (e - 1) / kListChunk;
+    if (e > s && c0 == c1) continue;  // finished by the chunk pass
+    const long long m = e > s ? c1 - c0 + 1 : 0;  // partials, in chunk order
+    long long cnt = 0;
+    for (long long j = threadIdx.x; j < m; j += kListThreads) cnt += pcnt[j == 0 ? 2 * c0 + 1 : 2 * (c0 + j)];
+    cnt = warp_sum(cnt);
+    if (lane_id() == 0) s_cnt[threadIdx.x >> 5] = cnt;
+    __syncthreads();
+    cnt = 0;
+    for (int w = 0; w < kListWarps; w++) cnt += s_cnt[w];
+    for (int cb = 0; cb < C; cb += Cw) {
+      const int c = cb + tx;
+      double sum = 0.0;
+      float mn = INFINITY, mx = -INFINITY;
+      if (c < C)
+        for (long long j = ty; j < m; j += rows_par) {
+          const size_t o = (size_t)(j == 0 ? 2 * c0 + 1 : 2 * (c0 + j)) * C + c;
+          sum += psum[o];
+          const float a = pmin[o], b = pmax[o];
+          mn = (a < mn) ? a : mn;
+          mx = (b > mx) ? b : mx;
+        }
+      s_sum[threadIdx.x] = sum;
+      s_min[threadIdx.x] = mn;
+      s_max[threadIdx.x] = mx;
+      __syncthreads();
+      for (int h = rows_par >> 1; h > 0; h >>= 1) {
+        if (ty < h) {
+          const int t = threadIdx.x + h * Cw;
+          s_sum[threadIdx.x] += s_sum[t];
+          s_min[threadIdx.x] = (s_min[t] < s_min[threadIdx.x]) ? s_min[t] : s_min[threadIdx.x];
+          s_max[threadIdx.x] = (s_max[t] > s_max[threadIdx.x]) ? s_max[t] : s_max[threadIdx.x];
+        }
+        __syncthreads();
+      }
+      if (ty == 0 && c < C) {
+        const size_t o = (size_t)k * C + c;
+        if (ops & SGB_REDUCE_MIN) omin[o] = s_min[tx];
+        if (ops & SGB_REDUCE_MAX) omax[o] = s_max[tx];
+        if (ops & SGB_REDUCE_MEAN) omean[o] = (float)(s_sum[tx] / (double)cnt);
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) ocnt[k] = cnt;
+  }
+}
+
+// (ordered confidence, ~k): the larger key is the higher confidence, then the smaller k. NaN orders below -inf and -0.0
+// equals +0.0. Key 0 is no list (~k >= 2^31 for every k < 2^31).
+__device__ __forceinline__ unsigned long long point_key(float conf, int k) {
+  uint32_t o = 0u;
+  if (!isnan(conf)) {
+    const uint32_t u = __float_as_uint(conf == 0.f ? 0.f : conf);
+    o = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+  }
+  return ((unsigned long long)o << 32) | (unsigned long long)(~(uint32_t)k);
+}
+
+__global__ void __launch_bounds__(kListThreads, kListCtasPerSm) id_map_keys_kernel(const long long *__restrict__ off, int n,
+                                                                   const int32_t *__restrict__ ids, long long total, int N,
+                                                                   const float *__restrict__ conf,
+                                                                   unsigned long long *__restrict__ key) {
+  const int lane = lane_id();
+  const long long nch = (total + kListChunk - 1) / kListChunk;
+  for (long long ch = (long long)blockIdx.x * kListWarps + (threadIdx.x >> 5); ch < nch; ch += (long long)gridDim.x * kListWarps) {
+    const long long cs = ch * kListChunk, ce = min(cs + kListChunk, total);
+    int k = list_of(off, n, cs);
+    for (long long i = cs + lane; i < ce; i += 32) {
+      while (k < n - 1 && off[k + 1] <= i) k++;
+      if (i < off[k] || i >= off[k + 1]) continue;  // ids outside [offsets[0], offsets[n]) belong to no list
+      const int id = __ldg(&ids[i]);
+      if ((unsigned)id < (unsigned)N) atomicMax(&key[id], point_key(__ldg(&conf[k]), k));
+    }
+  }
+}
+
+__global__ void id_map_decode_kernel(const unsigned long long *__restrict__ key, int N, int32_t *__restrict__ map) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p < N) {
+    const unsigned long long v = key[p];
+    map[p] = v ? (int32_t)~(uint32_t)v : -1;
+  }
+}
+
 }  // namespace sgb
 
 using namespace sgb;
@@ -479,6 +667,68 @@ int sgb_class_bitmaps(const int64_t *d_labels, int N, const int32_t *d_row_of_la
   if (N == 0 || n_labels == 0) return SGB_OK;
   SGB_REQUIRE(d_labels && d_row_of_label, SGB_ERR_ARG, "class_bitmaps pointers");
   class_bitmaps_kernel<<<div_up(N, 256), 256, 0, st>>>(d_labels, N, d_row_of_label, n_labels, d_bitmaps, W, d_counts);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+static long long list_chunks(long long total) { return (std::max(total, 0ll) + kListChunk - 1) / kListChunk; }
+
+// grid of the chunk passes: one warp per chunk, as many CTAs as are resident at once (the warps loop over the rest)
+static int list_chunk_grid(long long total, int sms) {
+  return (int)std::min<long long>(div_up(list_chunks(total), kListWarps), (long long)kListCtasPerSm * sms);
+}
+
+size_t sgb_id_lists_reduce_workspace_bytes(long long total, int C) {
+  const size_t slots = 2 * (size_t)list_chunks(total), sc = slots * (size_t)std::max(C, 0);
+  return align_up(sc * 8) + 2 * align_up(sc * 4) + align_up(slots * 4) + 1024;
+}
+
+int sgb_id_lists_reduce(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_values,
+                        long long ld, int C, int ops, float *d_min, float *d_max, float *d_mean, long long *d_counts, void *d_ws,
+                        size_t ws_bytes, void *stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SGB_REQUIRE(n >= 0 && total >= 0 && N >= 0 && C >= 1 && ld >= C, SGB_ERR_ARG, "id_lists_reduce sizes");
+  SGB_REQUIRE(ops > 0 && (ops & ~(SGB_REDUCE_MIN | SGB_REDUCE_MAX | SGB_REDUCE_MEAN)) == 0, SGB_ERR_ARG, "id_lists_reduce ops");
+  if (n == 0) return SGB_OK;
+  SGB_REQUIRE((!(ops & SGB_REDUCE_MIN) || d_min) && (!(ops & SGB_REDUCE_MAX) || d_max) && (!(ops & SGB_REDUCE_MEAN) || d_mean),
+              SGB_ERR_ARG, "id_lists_reduce: null output for a requested op");
+  SGB_REQUIRE(d_offsets && d_counts && (total == 0 || (d_ids && (N == 0 || d_values))), SGB_ERR_ARG, "id_lists_reduce pointers");
+  SGB_CURRENT_DEVICE(d);
+  const size_t sc = 2 * (size_t)list_chunks(total) * C;
+  Arena a(d_ws, ws_bytes);
+  double *psum = a.take<double>(sc);
+  float *pmin = a.take<float>(sc), *pmax = a.take<float>(sc);
+  int32_t *pcnt = a.take<int32_t>(2 * (size_t)list_chunks(total));
+  SGB_REQUIRE(psum && pmin && pmax && pcnt, SGB_ERR_WORKSPACE, "id_lists_reduce workspace too small");
+  if (total > 0) {
+    id_reduce_chunks_kernel<<<list_chunk_grid(total, d->sms), kListThreads, 0, st>>>(
+        d_offsets, n, d_ids, total, N, d_values, ld, C, ops, d_min, d_max, d_mean, d_counts, psum, pmin, pmax, pcnt);
+    SGB_LAUNCH_CHECK();
+  }
+  id_reduce_lists_kernel<<<std::min(n, 8 * d->sms), kListThreads, 0, st>>>(d_offsets, n, total, C, ops, psum, pmin, pmax, pcnt,
+                                                                          d_min, d_max, d_mean, d_counts);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+size_t sgb_id_lists_point_map_workspace_bytes(int N) { return align_up((size_t)std::max(N, 0) * 8) + 1024; }
+
+int sgb_id_lists_point_map(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_conf,
+                           int32_t *d_map, void *d_ws, size_t ws_bytes, void *stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SGB_REQUIRE(n >= 0 && total >= 0 && N >= 0, SGB_ERR_ARG, "id_lists_point_map sizes");
+  if (N == 0) return SGB_OK;
+  SGB_REQUIRE(d_map && (n == 0 || total == 0 || (d_offsets && d_ids && d_conf)), SGB_ERR_ARG, "id_lists_point_map pointers");
+  SGB_CURRENT_DEVICE(d);
+  Arena a(d_ws, ws_bytes);
+  unsigned long long *key = a.take<unsigned long long>((size_t)N);
+  SGB_REQUIRE(key, SGB_ERR_WORKSPACE, "id_lists_point_map workspace too small");
+  SGB_CUDA_CHECK(cudaMemsetAsync(key, 0, (size_t)N * 8, st));
+  if (n > 0 && total > 0) {
+    id_map_keys_kernel<<<list_chunk_grid(total, d->sms), kListThreads, 0, st>>>(d_offsets, n, d_ids, total, N, d_conf, key);
+    SGB_LAUNCH_CHECK();
+  }
+  id_map_decode_kernel<<<div_up(N, 256), 256, 0, st>>>(key, N, d_map);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

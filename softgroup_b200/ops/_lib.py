@@ -83,6 +83,11 @@ SIGNATURES = {
     'sgb_bitmap_ids_count': (c_int, [_P, c_int, c_int, _P, _P, c_size_t, _P]),
     'sgb_bitmap_ids_fill': (c_int, [_P, c_int, c_int, _P, _P, c_size_t, _P]),
     'sgb_class_bitmaps': (c_int, [_P, c_int, _P, c_int, _P, c_int, _P, _P]),
+    'sgb_id_lists_reduce_workspace_bytes': (c_size_t, [c_longlong, c_int]),
+    'sgb_id_lists_reduce': (c_int, [_P, _P, c_int, c_longlong, c_int, _P, c_longlong, c_int, c_int, _P, _P, _P, _P, _P, c_size_t,
+                                    _P]),
+    'sgb_id_lists_point_map_workspace_bytes': (c_size_t, [c_int]),
+    'sgb_id_lists_point_map': (c_int, [_P, _P, c_int, c_longlong, c_int, _P, _P, _P, c_size_t, _P]),
     'sgb_affine3_f64': (c_int, [_P, _P, _P, c_int, _P]),
     'sgb_rle_format_ids': (c_longlong, [_P, _P, c_int, _P, c_longlong, _P]),
 }

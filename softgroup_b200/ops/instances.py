@@ -172,6 +172,64 @@ def class_bitmaps(labels, classes, n_points):
     return bm, counts
 
 
+REDUCE_OPS = {'min': 1, 'max': 2, 'mean': 4}  # SGB_REDUCE_* of include/sgb200.h
+
+
+def _id_lists(instances):
+    off, ids = instances['point_offsets'], instances['point_ids']
+    assert off.is_cuda and off.dtype == torch.int64 and off.is_contiguous() and off.dim() == 1 and off.numel() >= 1
+    assert ids.is_cuda and ids.dtype == torch.int32 and ids.is_contiguous() and ids.device == off.device
+    return off, ids, off.numel() - 1, ids.numel()
+
+
+def instance_point_reduce(instances, values, ops=('min', 'max', 'mean')):
+    """Per instance and channel, min / max / mean of `values` over the instance's points, without gathering them.
+
+    instances: the `instances` dict of forward_test(device_results=True) (or any int64 `point_offsets` [n + 1] and int32
+    `point_ids` [point_offsets[n]] on the GPU); values: float32 CUDA [N, C] indexed by point id, rows may be strided
+    (stride(1) == 1). Under lvl_fusion the lists already hold point ids (not voxel rows), so `values` are per point, like
+    the dict's `offset_preds`. Returns dict(op -> float32 [n, C] for each op asked for, counts -> int64 [n]). min / max are
+    exact (NaN never wins; an empty instance gives +inf / -inf); mean has the same bits on every run, within the bound
+    stated in include/sgb200.h (sgb_id_lists_reduce), NaN for an empty instance. Enqueued on the current stream, no host
+    wait. Example, boxes and centroids: r = instance_point_reduce(inst, coords_float); r['min'], r['max'], r['mean']."""
+    off, ids, n, total = _id_lists(instances)
+    assert values.is_cuda and values.dtype == torch.float32 and values.dim() == 2 and values.device == off.device
+    assert values.size(1) >= 1 and (values.stride(1) == 1 or values.size(1) == 1)
+    ops = tuple(ops)
+    assert ops and all(o in REDUCE_OPS for o in ops) and len(set(ops)) == len(ops), ops
+    N, C = values.shape
+    ld = values.stride(0) if N > 1 else C
+    dev = off.device
+    out = {o: torch.empty((n, C), dtype=torch.float32, device=dev) for o in ops}
+    out['counts'] = torch.empty(n, dtype=torch.int64, device=dev)
+    L = _lib.lib()
+    ws = _ws(L.sgb_id_lists_reduce_workspace_bytes(total, C), dev)
+    with profiler.record('id_lists_reduce', 8 * (n + 1) + 4 * total + 4 * C * total + 4 * C * n * len(ops)):
+        check(L.sgb_id_lists_reduce(ptr(off), ptr(ids), n, total, N, ptr(values), ld, C, sum(REDUCE_OPS[o] for o in ops),
+                                    ptr(out.get('min')), ptr(out.get('max')), ptr(out.get('mean')), ptr(out['counts']), ptr(ws),
+                                    ws.numel(), _stream()), 'sgb_id_lists_reduce')
+    return out
+
+
+def instance_point_map(instances, num_points):
+    """One instance per point: int32 CUDA [num_points], the k of the highest-confidence instance (instances['conf']) that
+    holds the point; ties go to the smaller k, a NaN confidence ranks below every number, a point in no instance gets -1.
+    Takes the `instances` dict of forward_test(device_results=True) (point ids, also under lvl_fusion). Enqueued on the
+    current stream, no host wait; the result does not depend on execution order."""
+    off, ids, n, total = _id_lists(instances)
+    conf = instances['conf']
+    assert conf.is_cuda and conf.dtype == torch.float32 and conf.is_contiguous() and conf.numel() == n
+    N = int(num_points)
+    dev = off.device
+    out = torch.empty(N, dtype=torch.int32, device=dev)
+    L = _lib.lib()
+    ws = _ws(L.sgb_id_lists_point_map_workspace_bytes(N), dev)
+    with profiler.record('id_lists_point_map', 8 * (n + 1) + 4 * n + 4 * total + 20 * N):
+        check(L.sgb_id_lists_point_map(ptr(off), ptr(ids), n, total, N, ptr(conf), ptr(out), ptr(ws), ws.numel(), _stream()),
+              'sgb_id_lists_point_map')
+    return out
+
+
 def panoptic_paste(bitmaps, order, cls_values, semantic_preds, skip_iou, n_points):
     """softgroup.py:606-632 on bitmaps: -> (panoptic_cls uint32-valued int64 [N], panoptic_ids int64 [N]) CUDA tensors."""
     dev = bitmaps.device
