@@ -372,6 +372,35 @@ size_t sgb_id_lists_point_map_workspace_bytes(int N);
 int sgb_id_lists_point_map(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_conf,
                            int32_t *d_map, void *d_ws, size_t ws_bytes, void *stream);
 
+/* sgb_id_lists_fps: farthest-point sampling of K >= 1 points per list (same lists as above), d_out int32 [n, K] (int64
+ * indexing: n * K may exceed 2^31). Points are d_xyz f32 [N, 3] rows (x, y, z at d_xyz[id * ld + 0..2], ld >= 3).
+ * For list k, positions i = 0 .. len-1 hold ids p_i; position i is valid when 0 <= p_i < N. Invalid ids are never
+ * dereferenced and never chosen.
+ *   1. No valid position: row k is all -1.
+ *   2. s_0 = the smallest valid position; d_i = +inf for every valid i.
+ *   3. For j = 1 .. K-1: for every valid i, d_i = minimum(d_i, dist(i, s_{j-1})), where a NaN operand gives NaN (as
+ *      np.minimum); s_j = the valid position with the largest d_i, a NaN ranking below every number, ties going to the
+ *      smaller position.
+ *   4. out[k, j] = p_{s_j}.
+ * dist is float32, every operation rounded to nearest, no contraction, in this order: dx = x_i - x_s, dy, dz, then
+ * (dx*dx + dy*dy) + dz*dz; numpy's float32 dx*dx + dy*dy + dz*dz gives the same bits. The argmax is a max over the 64-bit
+ * key (0 for NaN, else the bits of d + 1 : 0xFFFFFFFF - position), so the result does not depend on the reduction
+ * order. When a list has fewer distinct points than K, the tail repeats one position's id (s_0's when the points are
+ * finite), as the tie rule implies. A list of more than 2^31 - 1 positions is outside this contract: its row is -1.
+ * Granularity, by list length (positions, valid or not): up to SGB_FPS_WARP_MAX one warp, up to SGB_FPS_CTA_MAX one
+ * CTA, beyond that one 8-CTA thread-block cluster, which keeps up to SGB_FPS_CLUSTER_MAX positions on chip and streams
+ * longer lists from global memory every step (their d in the workspace). A bin pass sorts the lists into one queue per
+ * granularity; the three kernels have fixed grids and pull lists from their queue. Enqueued on `stream`, no host wait.
+ * Launches: SGB_FPS_LAUNCHES whatever the data (none when n = 0), after one memset.
+ * Workspace: sgb_id_lists_fps_workspace_bytes(n, total) = three int32 queues of n lists plus 4 bytes per id. */
+#define SGB_FPS_WARP_MAX 512
+#define SGB_FPS_CTA_MAX 8192
+#define SGB_FPS_CLUSTER_MAX 65536
+#define SGB_FPS_LAUNCHES 4
+size_t sgb_id_lists_fps_workspace_bytes(int n, long long total);
+int sgb_id_lists_fps(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_xyz,
+                     long long ld, int K, int32_t *d_out, void *d_ws, size_t ws_bytes, void *stream);
+
 /* Test-time transform of the reference dataloader, first step (softgroup/data/custom.py:87-107,162-164):
  * out[i, :] = xyz[i, :] @ m in float64 (xyz float32 [N,3] device, m float64 [3,3] row-major HOST, out float64 [N,3] device),
  * accumulated like the BLAS kernels numpy calls: fma(z, m2j, fma(y, m1j, x * m0j)). */

@@ -450,6 +450,371 @@ __global__ void id_map_decode_kernel(const unsigned long long *__restrict__ key,
   }
 }
 
+// ---- farthest-point sampling per id list (sgb_id_lists_fps) ----------------------------------------------------------
+// A bin pass sorts the lists by length into three queues; a persistent kernel per queue pulls lists from it: one warp,
+// one CTA or one 8-CTA cluster per list. A thread keeps kFpsR positions (x, y, z, d) in registers, and a float4
+// (x, y, z, id) copy of each in shared memory broadcasts the chosen point. Each step is one argmax of fps_key over the
+// list, so the result does not depend on the reduction order. Lists beyond the cluster's capacity stream their points
+// from global memory every step and keep d in the workspace.
+constexpr int kFpsR = 16;            // positions per thread
+constexpr int kFpsCtaThreads = 512;  // CTA and cluster paths
+constexpr int kFpsCtaWarps = kFpsCtaThreads / 32;
+constexpr int kFpsWarpLists = 8;     // warp path: lists in flight per CTA
+constexpr int kFpsCl = 8;            // CTAs per cluster (portable maximum)
+static_assert(SGB_FPS_WARP_MAX == 32 * kFpsR, "warp path capacity");
+static_assert(SGB_FPS_CTA_MAX == kFpsCtaThreads * kFpsR, "CTA path capacity");
+static_assert(SGB_FPS_CLUSTER_MAX == kFpsCl * SGB_FPS_CTA_MAX, "cluster path on-chip capacity");
+
+// (0 for NaN, else the bits of d + 1 : 0xFFFFFFFF - position): the larger key is the larger d, then the smaller position.
+// d is never negative, so its bits order like its value. A valid position's key is never 0 (positions < 2^31).
+__device__ __forceinline__ unsigned long long fps_key(float d, int pos) {
+  const uint32_t hi = isnan(d) ? 0u : __float_as_uint(d) + 1u;
+  return ((unsigned long long)hi << 32) | (unsigned long long)(0xFFFFFFFFu - (uint32_t)pos);
+}
+__device__ __forceinline__ int fps_pos(unsigned long long key) { return (int)(0xFFFFFFFFu - (uint32_t)key); }
+// The chosen point's d is 0 or NaN: every d is then 0 or NaN, the d of a point with d = 0 stays 0 (its coordinates and
+// the chosen point's are finite) and NaN stays NaN, so every later step chooses the same position.
+__device__ __forceinline__ bool fps_settled(unsigned long long key) { return (key >> 32) <= 1ull; }
+
+__device__ __forceinline__ float fps_dist(float x, float y, float z, float sx, float sy, float sz) {
+  const float dx = __fsub_rn(x, sx), dy = __fsub_rn(y, sy), dz = __fsub_rn(z, sz);
+  return __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+}
+__device__ __forceinline__ float fps_min(float d, float t) { return (t < d || t != t) ? t : d; }  // np.minimum: NaN wins
+__device__ __forceinline__ unsigned long long umax64(unsigned long long a, unsigned long long b) { return a > b ? a : b; }
+
+__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = umax64(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// every thread of the CTA gets the CTA's largest key; one barrier (s_cand is double-buffered by `phase`)
+__device__ __forceinline__ unsigned long long cta_max_u64(unsigned long long v, unsigned long long (*s_cand)[kFpsCtaWarps],
+                                                          int &phase) {
+  v = warp_max_u64(v);
+  unsigned long long *c = s_cand[phase++ & 1];
+  if (lane_id() == 0) c[threadIdx.x >> 5] = v;
+  __syncthreads();
+  return warp_max_u64(lane_id() < kFpsCtaWarps ? c[lane_id()] : 0ull);
+}
+
+// list k clamped to the id array; a negative length or one beyond 2^31 - 1 positions counts as no position
+__device__ __forceinline__ int fps_list(const long long *__restrict__ off, int k, long long total, long long &start) {
+  start = min(off[k], total);
+  const long long len = min(off[k + 1], total) - start;
+  return (len < 0 || len > 0x7FFFFFFFll) ? 0 : (int)len;
+}
+
+struct FpsRegs {
+  float x[kFpsR], y[kFpsR], z[kFpsR], d[kFpsR];
+  uint32_t valid;
+};
+
+// positions first + r * STRIDE below `end` into registers (d = +inf) and into s_pts[lfirst + r * STRIDE]; returns the
+// largest key of those, i.e. the smallest valid position (0 if none)
+template <int STRIDE>
+__device__ __forceinline__ unsigned long long fps_load(FpsRegs &p, const int32_t *__restrict__ ids, long long start, int first,
+                                                       int end, int N, const float *__restrict__ xyz, long long ld,
+                                                       float4 *s_pts, int lfirst) {
+  unsigned long long best = 0;
+  p.valid = 0;
+#pragma unroll
+  for (int r = 0; r < kFpsR; r++) {
+    const int pos = first + r * STRIDE;
+    p.x[r] = p.y[r] = p.z[r] = 0.f;
+    p.d[r] = INFINITY;
+    const int id = pos < end ? __ldg(&ids[start + pos]) : -1;
+    if ((unsigned)id < (unsigned)N) {
+      const float *q = xyz + (size_t)id * ld;
+      p.x[r] = __ldg(q);
+      p.y[r] = __ldg(q + 1);
+      p.z[r] = __ldg(q + 2);
+      p.valid |= 1u << r;
+      s_pts[lfirst + r * STRIDE] = make_float4(p.x[r], p.y[r], p.z[r], __int_as_float(id));
+      best = umax64(best, fps_key(INFINITY, pos));
+    }
+  }
+  return best;
+}
+
+// one step over the registers: d = min(d, dist to s), returns the largest key
+template <int STRIDE>
+__device__ __forceinline__ unsigned long long fps_sweep(FpsRegs &p, int first, float sx, float sy, float sz) {
+  unsigned long long best = 0;
+#pragma unroll
+  for (int r = 0; r < kFpsR; r++) {
+    if (p.valid & (1u << r)) {
+      p.d[r] = fps_min(p.d[r], fps_dist(p.x[r], p.y[r], p.z[r], sx, sy, sz));
+      best = umax64(best, fps_key(p.d[r], first + r * STRIDE));
+    }
+  }
+  return best;
+}
+
+// Warp path (T = 32: kFpsWarpLists lists per CTA, one per warp, shuffles only) and CTA path (T = kFpsCtaThreads: one list
+// per CTA, one barrier per step). Positions are t + r * T, so a position's shared-memory slot is the position itself.
+template <int T>
+__global__ void __launch_bounds__(T == 32 ? 32 * kFpsWarpLists : T, T == 32 ? 2 : 1)
+    fps_lists_kernel(const long long *__restrict__ off, const int32_t *__restrict__ ids, long long total, int N,
+                     const float *__restrict__ xyz, long long ld, int K, const int32_t *__restrict__ queue,
+                     const int *__restrict__ count, int *head, int32_t *__restrict__ out) {
+  extern __shared__ float4 s_pts_all[];  // [lists per CTA][T * kFpsR]
+  __shared__ unsigned long long s_cand[2][kFpsCtaWarps];
+  __shared__ int s_item;
+  const int t = threadIdx.x % T;
+  float4 *s_pts = s_pts_all + (threadIdx.x / T) * (T * kFpsR);
+  const int n_items = *count;
+  int phase = 0;
+  FpsRegs p;
+  auto group_max = [&](unsigned long long v) {
+    if constexpr (T == 32) {
+      __syncwarp();  // s_pts stores before the broadcast read
+      return warp_max_u64(v);
+    } else {
+      return cta_max_u64(v, s_cand, phase);
+    }
+  };
+  while (true) {
+    int item;
+    if constexpr (T == 32) {
+      __syncwarp();  // the previous list's s_pts reads before this list's stores
+      item = __shfl_sync(0xffffffffu, t == 0 ? atomicAdd(head, 1) : 0, 0);
+    } else {
+      if (t == 0) s_item = atomicAdd(head, 1);
+      __syncthreads();
+      item = s_item;
+    }
+    if (item >= n_items) break;
+    const int k = queue[item];
+    long long start;
+    const int len = fps_list(off, k, total, start);
+    int32_t *row = out + (size_t)k * K;
+    unsigned long long best = group_max(fps_load<T>(p, ids, start, t, len, N, xyz, ld, s_pts, t));
+    if (best == 0) {  // no valid position
+      for (int j = t; j < K; j += T) row[j] = -1;
+      continue;
+    }
+    for (int j = 0;; j++) {
+      const float4 s = s_pts[fps_pos(best)];
+      const int id = __float_as_int(s.w);
+      if (j == K - 1 || fps_settled(best)) {
+        for (int jj = j + t; jj < K; jj += T) row[jj] = id;
+        break;
+      }
+      if (t == 0) row[j] = id;
+      best = group_max(fps_sweep<T>(p, t, s.x, s.y, s.z));
+    }
+  }
+}
+
+// streaming: positions first, first + kFpsCtaThreads, ... below `end`, points read from global memory, d from dws
+// (written, not read, on the first update, where the old d is +inf)
+__device__ __forceinline__ unsigned long long fps_stream_sweep(const int32_t *__restrict__ ids, long long start, int first, int end,
+                                                               int N, const float *__restrict__ xyz, long long ld,
+                                                               float *__restrict__ dws, bool first_update, float sx, float sy,
+                                                               float sz) {
+  constexpr int B = 4;  // loads in flight per thread
+  unsigned long long best = 0;
+  for (int pos0 = first; pos0 < end; pos0 += B * kFpsCtaThreads) {
+    int id[B];
+    float x[B], y[B], z[B], d[B];
+#pragma unroll
+    for (int b = 0; b < B; b++) {
+      const int pos = pos0 + b * kFpsCtaThreads;
+      id[b] = pos < end ? __ldg(&ids[start + pos]) : -1;
+    }
+#pragma unroll
+    for (int b = 0; b < B; b++) {
+      x[b] = y[b] = z[b] = 0.f;
+      d[b] = INFINITY;
+      if ((unsigned)id[b] < (unsigned)N) {
+        const float *q = xyz + (size_t)id[b] * ld;
+        x[b] = __ldg(q);
+        y[b] = __ldg(q + 1);
+        z[b] = __ldg(q + 2);
+        if (!first_update) d[b] = __ldcg(&dws[start + pos0 + b * kFpsCtaThreads]);
+      }
+    }
+#pragma unroll
+    for (int b = 0; b < B; b++) {
+      if ((unsigned)id[b] < (unsigned)N) {
+        const int pos = pos0 + b * kFpsCtaThreads;
+        d[b] = fps_min(d[b], fps_dist(x[b], y[b], z[b], sx, sy, sz));
+        __stcg(&dws[start + pos], d[b]);
+        best = umax64(best, fps_key(d[b], pos));
+      }
+    }
+  }
+  return best;
+}
+
+// the smallest valid position of first, first + kFpsCtaThreads, ... below `end`, as a key with d = +inf (0 if none)
+__device__ __forceinline__ unsigned long long fps_stream_first(const int32_t *__restrict__ ids, long long start, int first, int end,
+                                                               int N) {
+  for (int pos = first; pos < end; pos += kFpsCtaThreads)
+    if ((unsigned)__ldg(&ids[start + pos]) < (unsigned)N) return fps_key(INFINITY, pos);
+  return 0ull;
+}
+
+__device__ __forceinline__ void fps_cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t fps_cluster_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t fps_mapa(const void *p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"((uint32_t)__cvta_generic_to_shared(p)), "r"(rank));
+  return r;
+}
+
+struct alignas(16) FpsPick {
+  float x, y, z;
+  int id;
+  unsigned long long key;
+};
+
+// Cluster path: one list per 8-CTA cluster, CTA r owns the positions [r * slice, (r + 1) * slice). Per step each CTA
+// publishes its best (key, x, y, z, id) in its own shared memory (double-buffered), one barrier.cluster, then lanes 0..7
+// of every warp read the 8 candidates through distributed shared memory and reduce them identically.
+__global__ void __cluster_dims__(kFpsCl, 1, 1) __launch_bounds__(kFpsCtaThreads, 1)
+    fps_cluster_kernel(const long long *__restrict__ off, const int32_t *__restrict__ ids, long long total, int N,
+                       const float *__restrict__ xyz, long long ld, int K, const int32_t *__restrict__ queue,
+                       const int *__restrict__ count, int *head, float *__restrict__ dws, int32_t *__restrict__ out) {
+  extern __shared__ float4 s_pts[];  // [SGB_FPS_CTA_MAX]
+  __shared__ unsigned long long s_cand[2][kFpsCtaWarps];
+  __shared__ FpsPick s_pub[2];
+  __shared__ int s_item;
+  const int t = threadIdx.x, lane = lane_id();
+  const uint32_t crank = fps_cluster_rank();
+  const int n_items = *count;
+  int phase = 0, cphase = 0;
+  FpsRegs p;
+  while (true) {
+    if (crank == 0 && t == 0) s_item = atomicAdd(head, 1);
+    fps_cluster_sync();
+    int item;
+    asm volatile("ld.shared::cluster.s32 %0, [%1];" : "=r"(item) : "r"(fps_mapa(&s_item, 0)) : "memory");
+    if (item >= n_items) break;
+    const int k = queue[item];
+    long long start;
+    const int len = fps_list(off, k, total, start);
+    const int slice = (len + kFpsCl - 1) / kFpsCl;
+    const int a = (int)crank * slice, b = min(a + slice, len);
+    const bool stream = len > SGB_FPS_CLUSTER_MAX;
+    int32_t *row = out + (size_t)k * K;
+    auto pick = [&](unsigned long long v) {
+      v = cta_max_u64(v, s_cand, phase);
+      FpsPick *pub = &s_pub[cphase++ & 1];
+      if (t == 0) {
+        FpsPick m{0.f, 0.f, 0.f, -1, v};
+        if (v) {
+          const int pos = fps_pos(v);
+          if (!stream) {
+            const float4 s = s_pts[pos - a];
+            m.x = s.x, m.y = s.y, m.z = s.z, m.id = __float_as_int(s.w);
+          } else {
+            m.id = __ldg(&ids[start + pos]);
+            const float *q = xyz + (size_t)m.id * ld;
+            m.x = __ldg(q), m.y = __ldg(q + 1), m.z = __ldg(q + 2);
+          }
+        }
+        *pub = m;
+      }
+      fps_cluster_sync();
+      unsigned long long key = 0ull;
+      float x = 0.f, y = 0.f, z = 0.f, id = 0.f;
+      if (lane < kFpsCl) {
+        const uint32_t r = fps_mapa(pub, lane);
+        asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(x), "=f"(y), "=f"(z), "=f"(id) : "r"(r) : "memory");
+        asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(key) : "r"(r + 16) : "memory");
+      }
+      const unsigned long long top = warp_max_u64(key);
+      const int src = __ffs(__ballot_sync(0xffffffffu, lane < kFpsCl && key == top)) - 1;
+      return FpsPick{__shfl_sync(0xffffffffu, x, src), __shfl_sync(0xffffffffu, y, src), __shfl_sync(0xffffffffu, z, src),
+                     __float_as_int(__shfl_sync(0xffffffffu, id, src)), top};
+    };
+    FpsPick s = pick(stream ? fps_stream_first(ids, start, a + t, b, N)
+                            : fps_load<kFpsCtaThreads>(p, ids, start, a + t, b, N, xyz, ld, s_pts, t));
+    const int ct = (int)crank * kFpsCtaThreads + t;  // thread rank in the cluster
+    if (s.key == 0) {
+      for (int j = ct; j < K; j += kFpsCl * kFpsCtaThreads) row[j] = -1;
+      continue;
+    }
+    for (int j = 0;; j++) {
+      if (j == K - 1 || fps_settled(s.key)) {
+        for (int jj = j + ct; jj < K; jj += kFpsCl * kFpsCtaThreads) row[jj] = s.id;
+        break;
+      }
+      if (ct == 0) row[j] = s.id;
+      s = pick(stream ? fps_stream_sweep(ids, start, a + t, b, N, xyz, ld, dws, j == 0, s.x, s.y, s.z)
+                      : fps_sweep<kFpsCtaThreads>(p, a + t, s.x, s.y, s.z));
+    }
+  }
+  fps_cluster_sync();  // no CTA leaves while another may still read its shared memory
+}
+
+// lists -> queues[q][0 .. counts[q]): q = 0 for lengths up to SGB_FPS_WARP_MAX (and lengths with no position), 1 up to
+// SGB_FPS_CTA_MAX, 2 beyond. One atomic per warp and queue.
+__global__ void fps_bin_kernel(const long long *__restrict__ off, int n, long long total, int *__restrict__ counts,
+                               int32_t *__restrict__ queues) {
+  const int lane = lane_id();
+  for (long long base = (long long)blockIdx.x * blockDim.x; base < n; base += (long long)gridDim.x * blockDim.x) {
+    const int k = (int)(base + threadIdx.x);
+    int q = -1;
+    if (k < n) {
+      long long start;
+      const int len = fps_list(off, k, total, start);
+      q = len <= SGB_FPS_WARP_MAX ? 0 : (len <= SGB_FPS_CTA_MAX ? 1 : 2);
+    }
+    const unsigned peers = __match_any_sync(0xffffffffu, q);
+    const int leader = __ffs(peers) - 1;
+    int slot = 0;
+    if (lane == leader && q >= 0) slot = atomicAdd(&counts[q], __popc(peers));
+    slot = __shfl_sync(0xffffffffu, slot, leader) + __popc(peers & ((1u << lane) - 1u));
+    if (q >= 0) queues[(size_t)q * n + slot] = k;
+  }
+}
+
+// per device: dynamic shared memory of the three list kernels and their resident grids
+static DeviceOnce g_fps_once;
+static int g_fps_grid[kMaxDevices][3];
+constexpr size_t kFpsWarpSmem = (size_t)kFpsWarpLists * SGB_FPS_WARP_MAX * sizeof(float4);
+constexpr size_t kFpsCtaSmem = (size_t)SGB_FPS_CTA_MAX * sizeof(float4);
+
+static int fps_setup(Device *d) {
+  return once_per_device(g_fps_once, d->ordinal, [d] {
+    SGB_CUDA_CHECK(cudaFuncSetAttribute(fps_lists_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFpsWarpSmem));
+    SGB_CUDA_CHECK(cudaFuncSetAttribute(fps_lists_kernel<kFpsCtaThreads>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)kFpsCtaSmem));
+    SGB_CUDA_CHECK(cudaFuncSetAttribute(fps_cluster_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFpsCtaSmem));
+    int b0 = 0, b1 = 0, nc = 0;
+    SGB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b0, fps_lists_kernel<32>, 32 * kFpsWarpLists, kFpsWarpSmem));
+    SGB_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b1, fps_lists_kernel<kFpsCtaThreads>, kFpsCtaThreads,
+                                                                 kFpsCtaSmem));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(d->sms / kFpsCl * kFpsCl);
+    cfg.blockDim = dim3(kFpsCtaThreads);
+    cfg.dynamicSmemBytes = kFpsCtaSmem;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = kFpsCl;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    SGB_CUDA_CHECK(cudaOccupancyMaxActiveClusters(&nc, fps_cluster_kernel, &cfg));
+    SGB_REQUIRE(b0 >= 1 && b1 >= 1 && nc >= 1, SGB_ERR_CUDA, "id_lists_fps kernels do not fit on this device");
+    g_fps_grid[d->ordinal][0] = b0 * d->sms;
+    g_fps_grid[d->ordinal][1] = b1 * d->sms;
+    g_fps_grid[d->ordinal][2] = nc * kFpsCl;
+    return SGB_OK;
+  });
+}
+
 }  // namespace sgb
 
 using namespace sgb;
@@ -729,6 +1094,39 @@ int sgb_id_lists_point_map(const long long *d_offsets, const int32_t *d_ids, int
     SGB_LAUNCH_CHECK();
   }
   id_map_decode_kernel<<<div_up(N, 256), 256, 0, st>>>(key, N, d_map);
+  SGB_LAUNCH_CHECK();
+  return SGB_OK;
+}
+
+size_t sgb_id_lists_fps_workspace_bytes(int n, long long total) {
+  return align_up(16 * 4) + align_up(3 * (size_t)std::max(n, 0) * 4) + align_up((size_t)std::max(total, 0ll) * 4);
+}
+
+int sgb_id_lists_fps(const long long *d_offsets, const int32_t *d_ids, int n, long long total, int N, const float *d_xyz,
+                     long long ld, int K, int32_t *d_out, void *d_ws, size_t ws_bytes, void *stream) {
+  cudaStream_t st = (cudaStream_t)stream;
+  SGB_REQUIRE(n >= 0 && total >= 0 && N >= 0 && K >= 1 && ld >= 3, SGB_ERR_ARG, "id_lists_fps sizes");
+  if (n == 0) return SGB_OK;
+  SGB_REQUIRE(d_offsets && d_out && (total == 0 || d_ids) && (N == 0 || d_xyz), SGB_ERR_ARG, "id_lists_fps pointers");
+  SGB_CURRENT_DEVICE(d);
+  if (const int rc = fps_setup(d)) return rc;
+  Arena a(d_ws, ws_bytes);
+  int *counters = a.take<int>(16);  // counts[3], heads[3]
+  int32_t *queues = a.take<int32_t>(3 * (size_t)n);
+  float *dws = a.take<float>((size_t)total);
+  SGB_REQUIRE(counters && queues && dws, SGB_ERR_WORKSPACE, "id_lists_fps workspace too small");
+  const int *g = g_fps_grid[d->ordinal];
+  SGB_CUDA_CHECK(cudaMemsetAsync(counters, 0, 6 * 4, st));
+  fps_bin_kernel<<<std::min(div_up(n, 256), 4 * d->sms), 256, 0, st>>>(d_offsets, n, total, counters, queues);
+  SGB_LAUNCH_CHECK();
+  fps_cluster_kernel<<<g[2], kFpsCtaThreads, kFpsCtaSmem, st>>>(d_offsets, d_ids, total, N, d_xyz, ld, K, queues + 2 * (size_t)n,
+                                                              counters + 2, counters + 5, dws, d_out);
+  SGB_LAUNCH_CHECK();
+  fps_lists_kernel<kFpsCtaThreads><<<g[1], kFpsCtaThreads, kFpsCtaSmem, st>>>(d_offsets, d_ids, total, N, d_xyz, ld, K,
+                                                                             queues + (size_t)n, counters + 1, counters + 4, d_out);
+  SGB_LAUNCH_CHECK();
+  fps_lists_kernel<32><<<g[0], 32 * kFpsWarpLists, kFpsWarpSmem, st>>>(d_offsets, d_ids, total, N, d_xyz, ld, K, queues,
+                                                                        counters, counters + 3, d_out);
   SGB_LAUNCH_CHECK();
   return SGB_OK;
 }

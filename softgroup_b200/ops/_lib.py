@@ -88,6 +88,8 @@ SIGNATURES = {
                                     _P]),
     'sgb_id_lists_point_map_workspace_bytes': (c_size_t, [c_int]),
     'sgb_id_lists_point_map': (c_int, [_P, _P, c_int, c_longlong, c_int, _P, _P, _P, c_size_t, _P]),
+    'sgb_id_lists_fps_workspace_bytes': (c_size_t, [c_int, c_longlong]),
+    'sgb_id_lists_fps': (c_int, [_P, _P, c_int, c_longlong, c_int, _P, c_longlong, c_int, _P, _P, c_size_t, _P]),
     'sgb_affine3_f64': (c_int, [_P, _P, _P, c_int, _P]),
     'sgb_rle_format_ids': (c_longlong, [_P, _P, c_int, _P, c_longlong, _P]),
 }

@@ -211,6 +211,37 @@ def instance_point_reduce(instances, values, ops=('min', 'max', 'mean')):
     return out
 
 
+def instance_farthest_point_sample(instances, coords, num_samples):
+    """A fixed number of points per instance by farthest-point sampling: int32 CUDA [n, num_samples] of point ids.
+
+    instances: the `instances` dict of forward_test(device_results=True) (or any int64 `point_offsets` [n + 1] and int32
+    `point_ids` on the GPU); coords: float32 CUDA [N, 3] indexed by point id, rows may be strided (stride(1) == 1); under
+    lvl_fusion the lists hold point ids, so coords are per point (coords_float). num_samples (K): any int >= 1.
+
+    Semantics (include/sgb200.h, sgb_id_lists_fps): ids outside [0, N) are never read nor chosen; a list with no such id
+    gives a row of -1. The first sample is the list's first valid id. Every later one is the valid position farthest from
+    those chosen so far (min over them of the float32 squared distance, computed as (dx*dx + dy*dy) + dz*dz, rounded to
+    nearest with no contraction, NaN propagating); a NaN distance ranks below every number, and ties go to the smaller
+    position. A list with fewer distinct points than K repeats one id in its tail, as PointNet++ pads. The result does not
+    depend on execution order. Enqueued on the current stream, no host wait.
+    Example: ids = instance_farthest_point_sample(ret['instances'], coords_float, 1024); coords_float[ids.long()] is
+    [n, 1024, 3]."""
+    off, ids, n, total = _id_lists(instances)
+    assert coords.is_cuda and coords.dtype == torch.float32 and coords.dim() == 2 and coords.size(1) == 3
+    assert coords.stride(1) == 1 and coords.device == off.device
+    K = int(num_samples)
+    assert K >= 1, num_samples
+    N = coords.size(0)
+    ld = coords.stride(0) if N > 1 else 3
+    out = torch.empty((n, K), dtype=torch.int32, device=off.device)
+    L = _lib.lib()
+    ws = _ws(L.sgb_id_lists_fps_workspace_bytes(n, total), off.device)
+    with profiler.record('id_lists_fps', 8 * (n + 1) + 16 * total + 4 * n * K):
+        check(L.sgb_id_lists_fps(ptr(off), ptr(ids), n, total, N, ptr(coords), ld, K, ptr(out), ptr(ws), ws.numel(), _stream()),
+              'sgb_id_lists_fps')
+    return out
+
+
 def instance_point_map(instances, num_points):
     """One instance per point: int32 CUDA [num_points], the k of the highest-confidence instance (instances['conf']) that
     holds the point; ties go to the smaller k, a NaN confidence ranks below every number, a point in no instance gets -1.
