@@ -7,7 +7,10 @@
   * a constructed instance-branch case (`instance_case`) for the edges the workloads need not reach: more than 1000
     proposals (tiny U-Net batch items), single-point clusters and clusters flat in one or all axes (the cluster scale is
     inf, then clamped), clusters whose extent puts the scale at the clamp while their coordinates are far from the
-    origin, so that voxel coordinates land just below spatial_shape, and points shared by several proposals."""
+    origin, so that voxel coordinates land just below spatial_shape, and points shared by several proposals;
+  * the config cases (`CONFIG_CASES`, tests/test_gpu_forward_stages_configs.py) for the paths no bench workload takes:
+    lvl_fusion (scannet++) with every class at pyramid level 1 and with one class at level 2 from voxel rows, ScanNet200,
+    and pyramid level 3 (c5 with every thing point in one class)."""
 import collections
 import os
 import sys
@@ -18,7 +21,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import bench  # noqa: E402
+import forward_oracle as fo  # noqa: E402
+import oracle  # noqa: E402
 from softgroup_b200 import synth  # noqa: E402
 from softgroup_b200.configs import model_cfg  # noqa: E402
 from softgroup_b200.model import SoftGroup  # noqa: E402
@@ -61,6 +67,75 @@ def build_workload(case, seed=0):
     inj = synth.grouping_inputs(base, sigma=wl['sigma'], seed=seed, fragments=wl.get('fragments', 1),
                                 confusion=wl.get('confusion', 0.0))
     return dict(cfg=cfg, wl=wl, scan=sc, base=base, inj=inj, model=model)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the config cases
+# ---------------------------------------------------------------------------------------------------------------------
+# relabel: every thing point (instance label >= 0) carries this semantic class when the injection is drawn, so that one
+# class holds all of them (its instances stay apart: their offsets still point to their own centroids). level: the
+# pyramid level that class must take, or 1 for every class at level 1; None without a pyramid. from_grouping: the
+# backbone is not checked (the c5 workload case checks it on the same scan and weights).
+ConfigCase = collections.namedtuple('ConfigCase', 'name cfg shape relabel level min_classes from_grouping')
+CONFIG_CASES = [ConfigCase('pp_lvlfusion', 'scannet++', 'c2_scannet', None, 1, 1, False),
+                ConfigCase('pp_lvlfusion_l2', 'scannet++', 'c2_scannet', 17, 2, 1, False),
+                ConfigCase('scannet200', 'scannet200', 'c6_scannet200', None, None, 20, False),
+                ConfigCase('c5_level3', 'stpls3d++', 'c5_stpls3d', 9, 3, 1, True)]
+CONFIG_N_POINTS = 150000  # c5_level3 takes the c5 workload's scan
+
+
+def config_case(name):
+    return [c for c in CONFIG_CASES if c.name == name][0]
+
+
+def _relabelled(scan, c):
+    sc = dict(scan)
+    sem = scan['semantic_labels'].copy()
+    sem[scan['instance_labels'] >= 0] = c
+    sc['semantic_labels'] = sem
+    return sc
+
+
+def voxel_mean(a, v2p, num_voxels):
+    """The mean of every voxel's rows of a, summed in float64, as float32."""
+    v2p = np.asarray(v2p, np.int64)
+    cnt = np.bincount(v2p, minlength=num_voxels).astype(np.float64)
+    s = np.stack([np.bincount(v2p, weights=np.asarray(a, np.float64)[:, j], minlength=num_voxels)
+                  for j in range(a.shape[1])], 1)
+    return (s / cnt[:, None]).astype(np.float32)
+
+
+def class_counts(prob, cfg):
+    """Rows above score_thr of every class the grouping takes (not ignored, at least min_npoint rows)."""
+    g = cfg['grouping_cfg']
+    n = (np.asarray(prob) > np.float32(g['score_thr'])).sum(0)
+    return {c: int(n[c]) for c in range(cfg['semantic_classes'])
+            if c not in g['ignore_classes'] and n[c] >= cfg['test_cfg']['min_npoint']}
+
+
+def build_config_case(case, seed=0):
+    """Scan, injected point-wise predictions and model of a config case. Returns dict(cfg, scan: the host scan the
+    forward gets, model: CPU, inj: (scores, offsets) numpy on the rows the grouping takes, voxel rows under lvl_fusion,
+    v2p: the scan's v2p_map under lvl_fusion else None, counts: class_counts of the injection's float32 softmax).
+    Under lvl_fusion the heads' outputs are replaced by the injection averaged per voxel (the synthetic predictions
+    are per point); c5_level3 uses the c5 workload's scan, model and injection parameters."""
+    if case.name == 'c5_level3':
+        w = build_workload(workload_case('c5'), seed=seed)
+        cfg, scan, model, wl = w['cfg'], w['scan'], w['model'], w['wl']
+        inj = synth.grouping_inputs(_relabelled(w['base'], case.relabel), sigma=wl['sigma'], seed=seed)
+    else:
+        cfg = model_cfg(case.cfg)
+        torch.manual_seed(0)
+        model = SoftGroup(**cfg).eval()
+        scan = synth.make_scan(case.shape, seed=seed, n_points=CONFIG_N_POINTS)
+        src = scan if case.relabel is None else _relabelled(scan, case.relabel)
+        inj = synth.grouping_inputs(src, sigma=0.03, seed=seed)
+    v2p = None
+    if cfg['test_cfg'].get('lvl_fusion'):
+        vc, v2p, _ = oracle.voxelization_idx(scan['coords'], 1, 4)
+        inj = tuple(voxel_mean(a, v2p, vc.shape[0]) for a in inj)
+    prob = torch.from_numpy(inj[0]).softmax(-1).numpy()
+    return dict(cfg=cfg, scan=scan, model=model, inj=inj, v2p=v2p, counts=class_counts(prob, cfg))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -34,14 +34,16 @@ def merge_4_parts(x):
     return out
 
 
-def backbone(voxel_feats, voxel_coords, v2p_map, spatial_shape, sd, channels, num_blocks, x4_split=False):
+def backbone(voxel_feats, voxel_coords, v2p_map, spatial_shape, sd, channels, num_blocks, x4_split=False,
+             lvl_fusion=False):
     """softgroup.py:363-378 up to output_feats (point rows, float64 accumulation). With x4_split (:380-395) every piece
     (batch column k) runs through the U-Net as a batch of one, its rows go back to the voxel rows of that piece, and the
-    point rows are merged with merge_4_parts."""
+    point rows are merged with merge_4_parts. With lvl_fusion (:373-374) the voxel rows are returned: no v2p_map gather."""
     vc = np.asarray(voxel_coords).astype(np.int32)
     if not x4_split:
         out = so.backbone(voxel_feats, vc, spatial_shape, sd, channels, num_blocks, acc64=True)
-        return out[v2p_map]
+        return out if lvl_fusion else out[v2p_map]
+    assert not lvl_fusion, 'x4_split does not support lvl_fusion'  # :365
     out = np.zeros((vc.shape[0], channels), np.float32)
     for k in range(4):
         sel = np.flatnonzero(vc[:, 0] == k)
@@ -86,6 +88,16 @@ def _inv32(s):
     return torch.tensor(1.0, dtype=torch.float32) / torch.tensor(float(s), dtype=torch.float32)
 
 
+def _note(info, c, poff, level=None):
+    """info (a dict, when the caller passes one): 'classes', the class of every proposal in order, and 'levels', the
+    pyramid level of every class grouped."""
+    if info is None:
+        return
+    info.setdefault('classes', []).extend([c] * (len(poff) - 1))
+    if level is not None:
+        info.setdefault('levels', {})[c] = level
+
+
 def _append(idx_list, off_list, pidx, poff):
     """The merge of softgroup.py:466-473."""
     pidx = pidx.copy()
@@ -108,10 +120,10 @@ def _batch_offsets(batch_idxs, batch_size):
     return np.concatenate([[0], np.cumsum(np.bincount(batch_idxs, minlength=batch_size))]).astype(np.int32)
 
 
-def grouping(prob, pt_offsets, batch_idxs, coords_float, cfg, batch_size):
+def grouping(prob, pt_offsets, batch_idxs, coords_float, cfg, batch_size, info=None):
     """softgroup.py:412-480 without the pyramid: the per-class loop, ball query (bfs_cluster.cu:15-66, restated on a grid:
     oracle.ballquery_batch_p_grid) over the class's points of every batch item, then bfs_cluster (bfs_cluster.cpp:60-86).
-    prob: the softmax of the semantic scores (:422) as float32 [N, C]."""
+    prob: the softmax of the semantic scores (:422) as float32 [N, C]. info: see _note."""
     g, tc = cfg['grouping_cfg'], cfg['test_cfg']
     mean = np.asarray(g['class_numpoint_mean'], np.float32)
     batch_idxs = np.asarray(batch_idxs, np.int32)
@@ -127,6 +139,7 @@ def grouping(prob, pt_offsets, batch_idxs, coords_float, cfg, batch_size):
         nidx, sl = oracle.ballquery_batch_p_grid(xyz, b, _batch_offsets(b, batch_size), g['radius'])
         pidx, poff = oracle.bfs_cluster(mean, nidx, sl, g['npoint_thr'], c)
         pidx[:, 1] = obj[pidx[:, 1]]  # :464
+        _note(info, c, poff)
         _append(idx_list, off_list, pidx, poff)
     return _concat(idx_list, off_list)
 
@@ -136,12 +149,15 @@ def get_level(n):
     return 3 if n > 1000000 else 2 if n > 100000 else 1
 
 
-def grouping_pp(prob, pt_offsets, coords_float, cfg):
+def grouping_pp(prob, pt_offsets, coords_float, cfg, lvl_fusion=False, info=None):
     """SoftGroup++ grouping, batch size 1 (softgroup.py:412-507 with_pyramid + with_octree): per class the points are
     voxelised at base_size * level (pyramid_map :491-498, `.long()` truncation, mean of coords and offsets), the octree
     ball query (functions.py:14-44) runs at radius * level, bfs_cluster, and every point inherits the cluster of its
     level voxel (pyramid_inverse_map :500-507). The inverse map is built from the pairs: a level voxel is in at most one
-    cluster, and `nonzero()` of the dense matrix lists (cluster, point) pairs sorted by cluster, then point."""
+    cluster, and `nonzero()` of the dense matrix lists (cluster, point) pairs sorted by cluster, then point.
+    With lvl_fusion the rows are the scan's voxels (coords_float their mean coordinates, :332-334) and are pyramid
+    level 1 themselves: a level-1 class groups its rows directly at radius * 1, with neither pyramid map nor inverse map
+    (:447, :461); a class at a higher level re-voxelises the rows' mean coordinates. info: see _note."""
     g, tc = cfg['grouping_cfg'], cfg['test_cfg']
     mean = np.asarray(g['class_numpoint_mean'], np.float32)
     idx_list, off_list = [], []
@@ -153,6 +169,13 @@ def grouping_pp(prob, pt_offsets, coords_float, cfg):
             continue
         cf, po = coords_float[obj], pt_offsets[obj]
         level = get_level(obj.size)
+        if level == 1 and lvl_fusion:
+            nidx, sl = oracle.octree_ball_query((cf + po).astype(np.float32), g['mean_active'], g['radius'])
+            pidx, poff = oracle.bfs_cluster(mean, nidx, sl, g['npoint_thr'], c)
+            pidx[:, 1] = obj[pidx[:, 1]]
+            _note(info, c, poff, level)
+            _append(idx_list, off_list, pidx, poff)
+            continue
         # :492, a CUDA float32 tensor divided by a Python float: times the float32 reciprocal (see clusters_voxelization)
         q = cf * _inv32(g['pyramid_base_size'] * level).numpy()
         lc = np.concatenate([np.zeros((obj.size, 1), np.int64), np.trunc(q).astype(np.int64)], 1)
@@ -169,6 +192,7 @@ def grouping_pp(prob, pt_offsets, coords_float, cfg):
         pidx = np.stack([c_of_point[pts][order], pts[order]], 1).astype(np.int32)
         poff = np.concatenate([[0], np.cumsum(np.bincount(c_of_point[pts], minlength=n_cluster))]).astype(np.int32)
         pidx[:, 1] = obj[pidx[:, 1]]
+        _note(info, c, poff, level)
         _append(idx_list, off_list, pidx, poff)
     return _concat(idx_list, off_list)
 
@@ -242,36 +266,55 @@ def rle_from_ids(ids, length):
     return ' '.join(map(str, runs.tolist()))
 
 
-def get_instances(proposals_idx, semantic_scores, cls_scores, iou_scores, mask_scores, cfg):
+def voxel_points(voxels, v2p_map, num_voxels):
+    """The points of every listed voxel: returns (k int64, point int64), one row per (listed voxel voxels[k], point of
+    it), points of a voxel ascending."""
+    v2p = np.asarray(v2p_map, np.int64)
+    by_voxel = np.argsort(v2p, kind='stable')
+    cnt = np.bincount(v2p, minlength=num_voxels)
+    first = np.cumsum(cnt) - cnt
+    voxels = np.asarray(voxels, np.int64)
+    n = cnt[voxels]
+    k = np.repeat(np.arange(voxels.size), n)
+    within = np.arange(k.size) - np.repeat(np.cumsum(n) - n, n)
+    return k, by_voxel[first[voxels[k]] + within]
+
+
+def get_instances(proposals_idx, semantic_scores, cls_scores, iou_scores, mask_scores, cfg, v2p_map=None):
     """softgroup.py:538-604 from (proposal, point) pairs. Per instance class i (class-major, proposal order): a
     sem2ins class gives one instance of the points whose semantic argmax is i (conf 1); otherwise proposal p is kept iff
     softmax(cls)[p, i] > cls_score_thr and #{its points with mask_score[:, i] > mask_score_thr} >= min_npoint, its mask
-    being those points. Returns dict(keep bool [nP, nI], npoint int64 [nP, nI], score float64 [nP, nI],
-    cls_softmax float64 [nP, nI+1], instances = [(label_id, conf, rle counts)])."""
+    being those points. With v2p_map (lvl_fusion) proposals, scores and masks are on voxel rows: the masks are taken to
+    points through v2p_map (`mask_pred[:, v2p_map.long()]`, :560-561 and :579-580) before min_npoint counts them, so a
+    (proposal, voxel) entry stands for every point of its voxel. Returns dict(keep bool [nP, nI], npoint int64 [nP, nI]
+    (points), score float64 [nP, nI], cls_softmax float64 [nP, nI+1], semantic_preds int64 [N points],
+    instances = [(label_id, conf, rle counts over N points)])."""
     tc, nI, sem2ins = cfg['test_cfg'], cfg['instance_classes'], list(cfg['sem2ins_classes'])
-    N = semantic_scores.shape[0]
     nP = cls_scores.shape[0]
     pidx = np.asarray(proposals_idx, np.int64)
     cls_sm = softmax64(cls_scores)
     on = np.asarray(mask_scores)[:, :nI] > np.float32(tc['mask_score_thr'])  # :569 (float32 scores, float32 threshold)
+    sem_pred = np.asarray(semantic_scores).argmax(1)
+    if v2p_map is not None:
+        row, pts = voxel_points(pidx[:, 1], v2p_map, semantic_scores.shape[0])
+        pidx, on = np.stack([pidx[row, 0], pts], 1), on[row]
+        sem_pred = sem_pred[np.asarray(v2p_map, np.int64)]
+    N = sem_pred.shape[0]
     npoint = np.stack([np.bincount(pidx[:, 0], weights=on[:, i], minlength=nP) for i in range(nI)], 1).astype(np.int64)
     score = cls_sm[:, :nI] * np.clip(np.asarray(iou_scores, np.float64)[:, :nI], 0, 1)  # :567
     keep = (cls_sm[:, :nI] > tc['cls_score_thr']) & (npoint >= tc['min_npoint'])  # :574, :583-584
     keep[:, sem2ins] = False
     order = np.argsort(pidx[:, 0], kind='stable')
     start = np.concatenate([[0], np.cumsum(np.bincount(pidx[:, 0], minlength=nP))])
-    sem_pred = None
     instances = []
     for i in range(nI):
         if i in sem2ins:  # :556-561
-            if sem_pred is None:
-                sem_pred = np.asarray(semantic_scores).argmax(1)
             instances.append((i + 1, 1.0, rle_from_ids(np.flatnonzero(sem_pred == i), N)))
             continue
         for p in np.flatnonzero(keep[:, i]):
             rows = order[start[p]:start[p + 1]]
             instances.append((i + 1, score[p, i], rle_from_ids(pidx[rows[on[rows, i]], 1], N)))
-    return dict(keep=keep, npoint=npoint, score=score, cls_softmax=cls_sm, instances=instances)
+    return dict(keep=keep, npoint=npoint, score=score, cls_softmax=cls_sm, semantic_preds=sem_pred, instances=instances)
 
 
 def rle_decode(counts, length):

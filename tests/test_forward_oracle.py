@@ -4,7 +4,10 @@ tests/test_gpu_forward_stages.py trusts them:
     proposals, instance voxel data and the instances' RLE strings exactly, floats within the fixture's 2e-4;
   * the grid ball query (oracle.ballquery_batch_p_grid) returns the brute-force oracle's lists on the neighbour cases
     and on random ones (the 1000 cap, several batches, NaN / Inf points, pairs at exactly the radius);
-  * the case table follows bench.WORKLOADS, and the constructed instance case reaches every edge it is there for."""
+  * the case table follows bench.WORKLOADS, and the constructed instance case reaches every edge it is there for;
+  * the config cases reach the paths they are there for (lvl_fusion at pyramid levels 1 and 2, ScanNet200, level 3),
+    and the lvl_fusion paths of the restatement (grouping_pp on voxel rows, get_instances through v2p_map) equal the
+    dense restatements of tests/test_host_grouping.py and tests/test_host_instances.py."""
 import os
 import sys
 
@@ -177,6 +180,96 @@ def test_workload_cases_follow_bench():
     torch.manual_seed(0)
     ref = SoftGroup(**model_cfg(wl['cfg'])).eval().state_dict()
     assert all(torch.equal(v, ref[k]) for k, v in w['model'].state_dict().items())
+
+
+def test_config_cases_reach_their_paths():
+    """The table of forward_cases.CONFIG_CASES, from the injection alone (its float32 softmax on the CPU): pp_lvlfusion
+    groups every class at pyramid level 1 from voxel rows, pp_lvlfusion_l2 one class holding every thing voxel at level
+    2, scannet200 at least 20 classes, c5_level3 one class of 1.25M points at level 3."""
+    for case in fc.CONFIG_CASES:
+        w = fc.build_config_case(case)
+        cfg, scan, counts = w['cfg'], w['scan'], w['counts']
+        levels = {c: fo.get_level(n) for c, n in counts.items()}
+        inst, sem = scan['instance_labels'], scan['semantic_labels']
+        assert len(counts) >= case.min_classes, case.name
+        assert (w['v2p'] is not None) == bool(cfg['test_cfg'].get('lvl_fusion')), case.name
+        if w['v2p'] is not None:  # voxel rows, the injection their mean
+            vc, v2p, _ = oracle.voxelization_idx(scan['coords'], 1, 4)
+            assert np.array_equal(w['v2p'], v2p) and w['inj'][0].shape[0] == vc.shape[0] < scan['coords'].shape[0]
+            thing_voxels = np.unique(v2p[inst >= 0]).size
+        if case.name == 'pp_lvlfusion':
+            assert set(levels.values()) == {1} and len(levels) >= 10
+            assert np.unique(inst[np.isin(sem, list(counts)) & (inst >= 0)]).size >= 10
+        elif case.name == 'pp_lvlfusion_l2':
+            assert levels == {17: 2} and thing_voxels == 119638 and counts[17] > 100000
+        elif case.name == 'scannet200':
+            assert not cfg['grouping_cfg'].get('with_pyramid') and cfg['semantic_classes'] == 200
+            assert cfg['instance_classes'] == 198 and np.unique(sem[inst >= 0]).size >= 20
+        else:
+            assert case.name == 'c5_level3' and levels == {9: 3}
+            assert (inst >= 0).sum() == counts[9] == 1250073
+
+
+@pytest.mark.parametrize('lvl_fusion', [False, True])
+def test_grouping_pp_equals_dense_reference_loop(monkeypatch, lvl_fusion):
+    """grouping_pp against test_host_grouping's restatement with the dense [nCluster, n] inverse map, on a small scan
+    with classes at pyramid levels 1 and 2 (get_level scaled down on both sides). Under lvl_fusion both are fed voxel
+    rows: the scan's voxel-mean coordinates and the injection averaged per voxel."""
+    import test_host_grouping as thg
+    cfg = model_cfg('scannet++', channels=16, num_blocks=2, test_cfg=dict(min_npoint=30))
+    cfg['grouping_cfg'].update(class_numpoint_mean=[-1.] * 20, npoint_thr=10)  # components of >= 10 rows
+    model = SoftGroup(**cfg).eval()
+    sc = synth.make_scan('c2_scannet', seed=5, n_points=20000)
+    scores, offs = synth.grouping_inputs(sc, sigma=0.03, seed=5)
+    coords = sc['coords_float']
+    if lvl_fusion:
+        vc, v2p, p2v = oracle.voxelization_idx(sc['coords'], 1, 4)
+        scores, offs = (fc.voxel_mean(a, v2p, vc.shape[0]) for a in (scores, offs))
+        coords = oracle.voxelization(coords, p2v, 4)
+    prob = torch.from_numpy(scores).softmax(-1).numpy()
+    split = np.median(list(fc.class_counts(prob, cfg).values()))  # the larger classes at level 2
+    get_level = lambda n: 2 if n > split else 1  # noqa: E731
+    monkeypatch.setattr(fo, 'get_level', get_level)
+    model.get_level = get_level
+    bidx = np.zeros(scores.shape[0], np.int32)
+    want_idx, want_off = thg.reference_forward_grouping_pp(model, scores, offs, bidx, coords, lvl_fusion)
+    info = {}
+    got_idx, got_off = fo.grouping_pp(prob, offs, coords, cfg, lvl_fusion=lvl_fusion, info=info)
+    assert set(info['levels'].values()) == {1, 2} and want_off.size > 10
+    assert len(info['classes']) == got_off.size - 1 and info['classes'] == sorted(info['classes'])
+    assert np.array_equal(got_idx, want_idx) and np.array_equal(got_off, want_off)
+
+
+@pytest.mark.parametrize('name,seed', [('scannet', 3), ('s3dis', 4)])
+def test_get_instances_v2p_equals_dense_procedure(name, seed):
+    """get_instances(v2p_map=...) against test_host_instances' dense procedure under lvl_fusion: (proposal, voxel)
+    entries, masks taken to points, min_npoint counted in points (at a min_npoint where counting voxels would keep fewer
+    instances), sem2ins classes (s3dis) from the per-point semantic prediction."""
+    import test_host_instances as thi
+    thr = dict(min_npoint=40, cls_score_thr=0.02, mask_score_thr=-0.5)
+    cfg = model_cfg(name, test_cfg=thr)
+    nI, sem2ins = cfg['instance_classes'], cfg['sem2ins_classes']
+    n_vox, n_pts = 300, 1000
+    rng = np.random.RandomState(100 + seed)
+    v2p = rng.randint(0, n_vox, n_pts).astype(np.int32)  # some voxels hold several points, some none
+    pidx, sem, cls, iou, msk = thi._case(seed, n_vox, 12, cfg['semantic_classes'], nI)
+    want = thi.reference_get_instances('s', pidx, sem, cls, iou, msk, nI, sem2ins, thr['cls_score_thr'],
+                                       thr['mask_score_thr'], thr['min_npoint'], v2p_map=v2p.astype(np.int64),
+                                       lvl_fusion=True)
+    r = fo.get_instances(pidx, sem, cls, iou, msk, cfg, v2p_map=v2p)
+    got = r['instances']
+    assert len(got) == len(want) > len(sem2ins)
+    assert [x[0] for x in got] == [int(x['label_id']) for x in want]
+    assert [x[2] for x in got] == [x['pred_mask']['counts'] for x in want]
+    assert all(x['pred_mask']['length'] == n_pts for x in want)
+    conf_w = np.array([x['conf'] for x in want], np.float64)
+    assert np.all(np.abs(np.array([x[1] for x in got]) - conf_w) <= 1e-6 * np.abs(conf_w))
+    assert np.array_equal(r['semantic_preds'], sem.argmax(1)[v2p])
+    on = msk[:, :nI] > np.float32(thr['mask_score_thr'])
+    voxels = np.stack([np.bincount(pidx[:, 0], weights=on[:, i], minlength=cls.shape[0]) for i in range(nI)], 1)
+    cls_ok = fo.softmax64(cls)[:, :nI] > thr['cls_score_thr']
+    assert np.any(r['keep'] & (voxels < thr['min_npoint']))  # kept only because points are counted
+    assert np.array_equal(r['keep'], cls_ok & (r['npoint'] >= thr['min_npoint']) & ~np.isin(np.arange(nI), sem2ins))
 
 
 def test_instance_case_reaches_its_edges():

@@ -119,8 +119,9 @@ def _flips(gpu_on, want64, thr, err, what, rep):
     return flip
 
 
-def _check_instance_branch(rep, cfg, sd, rec, pidx, poff, feats, coords_float, sem_scores):
-    """clusters_voxelization -> tiny U-Net -> instance heads -> get_instances, each fed the GPU's input."""
+def _check_instance_branch(rep, cfg, sd, rec, pidx, poff, feats, coords_float, sem_scores, v2p_map=None):
+    """clusters_voxelization -> tiny U-Net -> instance heads -> get_instances, each fed the GPU's input. v2p_map
+    (lvl_fusion): the branch runs on voxel rows and get_instances takes its masks to points through it."""
     ivc = cfg['instance_voxel_cfg']
     a, kw, (inst_x, inst_map) = rec['clusters_voxelization']
     assert np.array_equal(a[0], pidx) and np.array_equal(a[1], poff)
@@ -140,34 +141,36 @@ def _check_instance_branch(rep, cfg, sd, rec, pidx, poff, feats, coords_float, s
     # get_instances on the GPU's scores
     ga, gkw, inst = rec['get_instances']
     _, p_idx, g_sem, g_cls, g_iou, g_mask = ga
-    r = rep.oracle(fo.get_instances, p_idx, g_sem, g_cls, g_iou, g_mask, cfg)
+    r = rep.oracle(fo.get_instances, p_idx, g_sem, g_cls, g_iou, g_mask, cfg, v2p_map=v2p_map)
     got = [(int(x['label_id']), float(x['conf']), x['pred_mask']['counts']) for x in inst]
     rep.exact('instances', dict(labels=([x[0] for x in got], [x[0] for x in r['instances']]),
                                 rle=([x[2] for x in got], [x[2] for x in r['instances']])))
     conf_g, conf_w = np.array([x[1] for x in got]), np.array([x[1] for x in r['instances']], np.float64)
     assert np.all(np.abs(conf_g - conf_w) <= CONF_REL * np.abs(conf_w)), rep.tag + ': confidences'
-    assert all(x['pred_mask']['length'] == g_sem.shape[0] for x in inst)
+    assert all(x['pred_mask']['length'] == r['semantic_preds'].shape[0] for x in inst)
     # decisions the float64 scores would take differently
     nI, tc = cfg['instance_classes'], cfg['test_cfg']
     on_gpu = g_mask[:, :nI] > np.float32(tc['mask_score_thr'])
     mflip = _flips(on_gpu, mask64[:, :nI], tc['mask_score_thr'], err_mask, 'mask_score > thr', rep)
-    r64 = fo.get_instances(p_idx, g_sem, cls64, iou64, mask64, cfg)
+    r64 = fo.get_instances(p_idx, g_sem, cls64, iou64, mask64, cfg, v2p_map=v2p_map)
     sm_err = float(np.abs(r64['cls_softmax'] - r['cls_softmax']).max()) + err_cls
     kflip = r['keep'] != r64['keep']
     by_cls = np.abs(r64['cls_softmax'][:, :nI] - tc['cls_score_thr']) <= sm_err
     nflip = np.zeros_like(r['npoint'])
+    # a flipped (proposal, voxel) decision moves npoint by the voxel's points under lvl_fusion
+    pts = 1 if v2p_map is None else np.bincount(v2p_map, minlength=g_sem.shape[0])[p_idx[:, 1]]
     for i in range(nI):
-        nflip[:, i] = np.bincount(p_idx[:, 0], weights=mflip[:, i], minlength=nflip.shape[0])
+        nflip[:, i] = np.bincount(p_idx[:, 0], weights=mflip[:, i] * pts, minlength=nflip.shape[0])
     by_mask = np.abs(r['npoint'] - r64['npoint']) <= nflip
     rep.note('%-22s %d flips of %d decisions' % ('keep', int(kflip.sum()), kflip.size))
     assert np.all(~kflip | by_cls | (by_mask & (nflip > 0))), rep.tag + ': keep flips away from the thresholds'
     return r
 
 
-def _check_device_only(rep, cfg, rec):
+def _check_device_only(rep, cfg, rec, v2p_map=None):
     ga, _, dev = rec['get_instances']
     _, p_idx, g_sem, g_cls, g_iou, g_mask = ga
-    r = rep.oracle(fo.get_instances, p_idx, g_sem, g_cls, g_iou, g_mask, cfg)
+    r = rep.oracle(fo.get_instances, p_idx, g_sem, g_cls, g_iou, g_mask, cfg, v2p_map=v2p_map)
     rep.exact('device_only keep/npoint', dict(keep=(dev['keep'], r['keep']), npoint=(dev['npoint'], r['npoint'])))
     # Scores of kept pairs (the confidences) within 1e-6. The others can be tiny: a float32 softmax value exp(x - max)
     # carries the rounding of x - max, a relative error ~2^-24 |x - max| (~1e-6 at probabilities ~1e-8), and values

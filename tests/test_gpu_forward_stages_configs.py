@@ -1,0 +1,146 @@
+"""The whole CUDA forward on the paths no bench workload takes (tests/forward_cases.CONFIG_CASES), stage by stage
+against the host restatement tests/forward_oracle.py, with the bars of tests/test_gpu_forward_stages.py:
+
+  * pp_lvlfusion, pp_lvlfusion_l2 (scannet++, lvl_fusion): the backbone returns voxel rows, the heads, the grouping and
+    the instance branch run on them, level-1 classes group the rows themselves (no pyramid map), and get_instances takes
+    (proposal, voxel) entries to points and counts points for min_npoint. The real backbone and heads are checked; their
+    outputs are then replaced by the synthetic predictions averaged per voxel. In pp_lvlfusion every class is at pyramid
+    level 1, in pp_lvlfusion_l2 one class holds every thing voxel and is re-voxelised at level 2 from voxel rows.
+    The device_only and device_results forms are checked as well: keep, npoint and score, and the point ids;
+  * scannet200: 200 semantic and 198 instance classes through the one-pass grouping;
+  * c5_level3: the c5 tile with every thing point in one class (1.25M points), grouped at pyramid level 3
+    (quantisation at 0.3333 * 3, octree query at radius 2.7, inverse map over the 1.25M points); checked from the
+    grouping on (the c5 case of tests/test_gpu_forward_stages.py checks the backbone on the same scan and weights).
+
+Run with -s for each case's stage table, its GPU and CPU oracle times and the pyramid level every class took."""
+import os
+import sys
+import time
+
+import numpy as np
+import pytest
+import torch
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import forward_cases as fc  # noqa: E402
+import forward_oracle as fo  # noqa: E402
+import oracle  # noqa: E402
+from test_gpu_forward_stages import CONF_REL, Report, _check_device_only, _check_instance_branch, _flips, _record, _sd  # noqa: E402
+from softgroup_b200 import harness, spconv  # noqa: E402
+
+pytestmark = pytest.mark.gpu
+
+
+def _check_device_results(rep, cfg, rec, dev, v2p_map):
+    """forward_test(device_results=True): every instance's point ids, ascending, its label and confidence, and the
+    per-point semantic predictions, against get_instances restated on the GPU's inputs of that forward."""
+    ga = rec['get_instances'][0]
+    _, p_idx, g_sem, g_cls, g_iou, g_mask = ga
+    r = rep.oracle(fo.get_instances, p_idx, g_sem, g_cls, g_iou, g_mask, cfg, v2p_map=v2p_map)
+    inst = {k: v.cpu().numpy() for k, v in dev['instances'].items()}
+    off, ids = inst['point_offsets'], inst['point_ids']
+    lists = [ids[off[k]:off[k + 1]] for k in range(off.size - 1)]
+    assert all(np.all(np.diff(x) > 0) for x in lists), rep.tag + ': device_results point ids not ascending'
+    n = r['semantic_preds'].shape[0]
+    rep.exact('device_results', dict(label_id=(inst['label_id'], [x[0] for x in r['instances']]),
+                                     point_ids=([fo.rle_from_ids(x, n) for x in lists], [x[2] for x in r['instances']]),
+                                     semantic_preds=(dev['semantic_preds'].cpu().numpy(), r['semantic_preds'])))
+    conf_w = np.array([x[1] for x in r['instances']], np.float64)
+    assert np.all(np.abs(inst['conf'] - conf_w) <= CONF_REL * np.abs(conf_w)), rep.tag + ': device_results confidences'
+
+
+@pytest.mark.parametrize('name', [c.name for c in fc.CONFIG_CASES])
+def test_config_forward_stages_vs_oracle(name, monkeypatch):
+    case = fc.config_case(name)
+    w = fc.build_config_case(case)
+    cfg, scan, v2p = w['cfg'], w['scan'], w['v2p']
+    lvl_fusion = v2p is not None
+    assert lvl_fusion == bool(cfg['test_cfg'].get('lvl_fusion')) and int(scan['batch_size']) == 1
+    model = w['model'].cuda()
+    sd = _sd(model)
+    hb = harness.to_host_batch(scan, pin=False)
+    inj = tuple(torch.from_numpy(a).cuda() for a in w['inj'])
+    rec = _record(monkeypatch, model)
+    run_kw = dict(inject_pointwise=inj)
+    if lvl_fusion:  # the real backbone and heads run (and are recorded); the grouping gets the voxel-averaged injection
+        recorded = model.forward_backbone
+
+        def voxel_heads(input, input_map, **kw):
+            feats = recorded(input, input_map, **kw)[2]
+            return inj[0], inj[1], feats
+
+        monkeypatch.setattr(model, 'forward_backbone', voxel_heads)
+        run_kw = {}
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    with torch.no_grad():
+        ret = harness.run_scan(model, hb, **run_kw)
+    torch.cuda.synchronize()
+    t_gpu = time.perf_counter() - t0
+    rep = Report(name)
+
+    fkw = rec['forward_test'][0]
+    (bx, bmap), bkw, (sem, off, ofeat) = rec['forward_backbone']
+    vc, v2p_o, p2v, vf = rep.oracle(fo.voxelize, scan['coords'], scan['feats'], scan['coords_float'], model.with_coords, 1)
+    rep.exact('voxelize', dict(voxel_coords=(fkw['voxel_coords'], vc), v2p=(fkw['v2p_map'], v2p_o), p2v=(fkw['p2v_map'], p2v),
+                               voxel_feats=(bx['features'], vf), indices=(bx['indices'], vc)))
+    assert bkw.get('lvl_fusion', False) == lvl_fusion
+    if not case.from_grouping:
+        out64 = rep.oracle(fo.backbone, bx['features'], bx['indices'], bmap, scan['spatial_shape'], sd, cfg['channels'],
+                           cfg['num_blocks'], lvl_fusion=lvl_fusion)
+        assert ofeat.shape[0] == (vc.shape[0] if lvl_fusion else v2p_o.shape[0])
+        rep.floats('backbone', ofeat, out64)
+        sem64, off64 = rep.oracle(fo.pointwise_heads, ofeat, sd)
+        rep.floats('semantic_linear', sem, sem64)
+        rep.floats('offset_linear', off, off64)
+
+    # grouping, fed its GPU inputs: voxel rows under lvl_fusion (mean coordinates, batch index of the voxel coords)
+    ga, gkw, (pidx, poff) = rec['forward_grouping']
+    g_sem, g_off, g_bidx, g_cf = ga[:4]
+    assert np.array_equal(g_sem, w['inj'][0]) and np.array_equal(g_off, w['inj'][1])
+    if lvl_fusion:
+        assert np.array_equal(v2p, v2p_o)  # the injection was averaged over the voxels the forward hashed
+        rep.exact('voxel rows', dict(coords_float=(g_cf, oracle.voxelization(scan['coords_float'], p2v, 4)),
+                                     batch_idxs=(g_bidx, vc[:, 0])))
+    else:
+        assert np.array_equal(g_cf, scan['coords_float'])
+    with torch.no_grad():
+        prob = torch.from_numpy(g_sem).cuda().softmax(-1).cpu().numpy()
+    p64 = fo.softmax64(g_sem)
+    rep.floats('softmax', prob, p64, bar=CONF_REL)
+    _flips(prob > np.float32(cfg['grouping_cfg']['score_thr']), p64, cfg['grouping_cfg']['score_thr'],
+           float(np.abs(prob - p64).max()), 'score > score_thr', rep)
+    info = {}
+    if cfg['grouping_cfg'].get('with_pyramid'):
+        want = rep.oracle(fo.grouping_pp, prob, g_off, g_cf, cfg, lvl_fusion=lvl_fusion, info=info)
+    else:
+        want = rep.oracle(fo.grouping, prob, g_off, g_bidx, g_cf, cfg, gkw['batch_size'], info=info)
+    rep.exact('grouping', dict(proposals_idx=(pidx, want[0]), proposals_offset=(poff, want[1])))
+    classes, levels = info.get('classes', []), info.get('levels', {})
+    assert len(classes) == len(poff) - 1
+    rep.note('%-22s %d proposals over %d classes, %d (proposal, %s) pairs' %
+             ('', len(poff) - 1, len(set(classes)), len(pidx), 'voxel' if lvl_fusion else 'point'))
+    if levels:
+        rep.note('%-22s pyramid levels %s' % ('', ', '.join('%d: %d' % kv for kv in sorted(levels.items()))))
+    assert len(poff) - 1 >= 10 and len(set(classes)) >= case.min_classes
+    assert levels == {c: fo.get_level(n) for c, n in w['counts'].items()} if case.level else not levels
+    if case.level == 1:
+        assert levels and set(levels.values()) == {1}
+    elif case.level:
+        assert levels == {case.relabel: case.level}
+
+    # instance branch
+    r = _check_instance_branch(rep, cfg, sd, rec, pidx, poff, ofeat, g_cf, g_sem, v2p_map=v2p)
+    rep.exact('semantic_preds', dict(semantic_preds=(ret['semantic_preds'], r['semantic_preds'])))
+    # the bench path: results stay on the device
+    with torch.no_grad():
+        harness.run_scan(model, hb, device_only=True, **run_kw)
+    spconv.check_overflow()
+    _check_device_only(rep, cfg, rec, v2p_map=v2p)
+    if lvl_fusion:
+        with torch.no_grad():
+            dev = harness.run_scan(model, hb, device_results=True, **run_kw)
+        torch.cuda.synchronize()
+        spconv.check_overflow()
+        _check_device_results(rep, cfg, rec, dev, v2p)
+    rep.show(t_gpu)
