@@ -119,6 +119,18 @@ def ballquery_batch_p_grid(coords, batch_idxs, batch_offsets, radius):
     return idx[:tot], start_len
 
 
+def ballquery_total_grid(coords, batch_idxs, batch_offsets, radius):
+    """The neighbour total of ballquery_batch_p_grid (the sum of its list lengths) without writing the lists."""
+    coords = _c(coords, np.float32)
+    batch_idxs = _c(batch_idxs, np.int32)
+    batch_offsets = _c(batch_offsets, np.int32)
+    n = coords.shape[0]
+    start_len = np.zeros((n, 2), np.int32)
+    return int(lib().orc_ballquery_batch_p_grid(_p(coords, _f32p), _p(batch_idxs, _i32p), _p(batch_offsets, _i32p),
+                                                batch_offsets.shape[0] - 1, n, ctypes.c_float(radius), None,
+                                                ctypes.c_longlong(0), _p(start_len, _i32p)))
+
+
 def bfs_cluster(cluster_numpoint_mean, ball_query_idxs, start_len, threshold, class_id):
     """functions.py:278-308 -> (cluster_idxs i32 [sumNPoint,2], cluster_offsets i32 [nCluster+1])."""
     mean = _c(cluster_numpoint_mean, np.float32)

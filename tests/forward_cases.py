@@ -10,7 +10,10 @@
     origin, so that voxel coordinates land just below spatial_shape, and points shared by several proposals;
   * the config cases (`CONFIG_CASES`, tests/test_gpu_forward_stages_configs.py) for the paths no bench workload takes:
     lvl_fusion (scannet++) with every class at pyramid level 1 and with one class at level 2 from voxel rows, ScanNet200,
-    and pyramid level 3 (c5 with every thing point in one class)."""
+    pyramid level 3 (c5 with every thing point in one class), SoftGroup++ S3DIS (lvl_fusion with sem2ins classes on the
+    whole 800k-point room, one merged class at level 2) and the plain SoftGroup STPLS3D config (the c5 tile through a
+    one-pass ball query of 1.24e9 neighbours). On one H100 the two last took 1.14 s and 0.59 s of GPU forward and
+    192 s and 134 s of CPU oracle."""
 import collections
 import os
 import sys
@@ -72,26 +75,38 @@ def build_workload(case, seed=0):
 # ---------------------------------------------------------------------------------------------------------------------
 # the config cases
 # ---------------------------------------------------------------------------------------------------------------------
+# n_points: the scan's size (shape at seed 0), or None for the c5 workload's scan, injection parameters and weights.
 # relabel: every thing point (instance label >= 0) carries this semantic class when the injection is drawn, so that one
-# class holds all of them (its instances stay apart: their offsets still point to their own centroids). level: the
-# pyramid level that class must take, or 1 for every class at level 1; None without a pyramid. from_grouping: the
-# backbone is not checked (the c5 workload case checks it on the same scan and weights).
-ConfigCase = collections.namedtuple('ConfigCase', 'name cfg shape relabel level min_classes from_grouping')
-CONFIG_CASES = [ConfigCase('pp_lvlfusion', 'scannet++', 'c2_scannet', None, 1, 1, False),
-                ConfigCase('pp_lvlfusion_l2', 'scannet++', 'c2_scannet', 17, 2, 1, False),
-                ConfigCase('scannet200', 'scannet200', 'c6_scannet200', None, None, 20, False),
-                ConfigCase('c5_level3', 'stpls3d++', 'c5_stpls3d', 9, 3, 1, True)]
-CONFIG_N_POINTS = 150000  # c5_level3 takes the c5 workload's scan
+# class holds all of them (its instances stay apart: their offsets still point to their own centroids); a pair (a, b):
+# the thing points of class a carry class b, so b holds the things of both. level: the pyramid level that class must
+# take (every other class at level 1), or 1 for every class at level 1; None without a pyramid. min_classes: the
+# classes with proposals, at least. from_grouping: the backbone is not checked (the c5 workload case checks it on the
+# same scan and weights).
+ConfigCase = collections.namedtuple('ConfigCase', 'name cfg shape n_points relabel level min_classes from_grouping')
+CONFIG_CASES = [ConfigCase('pp_lvlfusion', 'scannet++', 'c2_scannet', 150000, None, 1, 1, False),
+                ConfigCase('pp_lvlfusion_l2', 'scannet++', 'c2_scannet', 150000, 17, 2, 1, False),
+                ConfigCase('scannet200', 'scannet200', 'c6_scannet200', 150000, None, None, 20, False),
+                ConfigCase('c5_level3', 'stpls3d++', 'c5_stpls3d', None, 9, 3, 1, True),
+                ConfigCase('s3dis_pp', 's3dis++', 'c3_s3dis', 800000, (7, 5), 2, 9, False),
+                ConfigCase('stpls3d', 'stpls3d', 'c5_stpls3d', None, None, None, 10, True)]
 
 
 def config_case(name):
     return [c for c in CONFIG_CASES if c.name == name][0]
 
 
-def _relabelled(scan, c):
+def relabel_target(case):
+    """The class that holds the relabelled thing points, or None."""
+    return case.relabel[1] if isinstance(case.relabel, tuple) else case.relabel
+
+
+def _relabelled(scan, relabel):
     sc = dict(scan)
     sem = scan['semantic_labels'].copy()
-    sem[scan['instance_labels'] >= 0] = c
+    if isinstance(relabel, tuple):
+        sem[(scan['instance_labels'] >= 0) & (sem == relabel[0])] = relabel[1]
+    else:
+        sem[scan['instance_labels'] >= 0] = relabel
     sc['semantic_labels'] = sem
     return sc
 
@@ -118,16 +133,23 @@ def build_config_case(case, seed=0):
     forward gets, model: CPU, inj: (scores, offsets) numpy on the rows the grouping takes, voxel rows under lvl_fusion,
     v2p: the scan's v2p_map under lvl_fusion else None, counts: class_counts of the injection's float32 softmax).
     Under lvl_fusion the heads' outputs are replaced by the injection averaged per voxel (the synthetic predictions
-    are per point); c5_level3 uses the c5 workload's scan, model and injection parameters."""
-    if case.name == 'c5_level3':
+    are per point); c5_level3 and stpls3d use the c5 workload's scan and injection parameters, and its weights."""
+    if case.n_points is None:
         w = build_workload(workload_case('c5'), seed=seed)
         cfg, scan, model, wl = w['cfg'], w['scan'], w['model'], w['wl']
-        inj = synth.grouping_inputs(_relabelled(w['base'], case.relabel), sigma=wl['sigma'], seed=seed)
+        if case.cfg != 'stpls3d++':  # the same module tree, hence the same weights: the c5 case checks its backbone
+            cfg = model_cfg(case.cfg)
+            torch.manual_seed(0)
+            model = SoftGroup(**cfg).eval()
+            sd, sd5 = model.state_dict(), w['model'].state_dict()
+            assert list(sd) == list(sd5) and all(torch.equal(v, sd5[k]) for k, v in sd.items()), case.name
+        src = w['base'] if case.relabel is None else _relabelled(w['base'], case.relabel)
+        inj = synth.grouping_inputs(src, sigma=wl['sigma'], seed=seed)
     else:
         cfg = model_cfg(case.cfg)
         torch.manual_seed(0)
         model = SoftGroup(**cfg).eval()
-        scan = synth.make_scan(case.shape, seed=seed, n_points=CONFIG_N_POINTS)
+        scan = synth.make_scan(case.shape, seed=seed, n_points=case.n_points)
         src = scan if case.relabel is None else _relabelled(scan, case.relabel)
         inj = synth.grouping_inputs(src, sigma=0.03, seed=seed)
     v2p = None

@@ -123,7 +123,8 @@ def _batch_offsets(batch_idxs, batch_size):
 def grouping(prob, pt_offsets, batch_idxs, coords_float, cfg, batch_size, info=None):
     """softgroup.py:412-480 without the pyramid: the per-class loop, ball query (bfs_cluster.cu:15-66, restated on a grid:
     oracle.ballquery_batch_p_grid) over the class's points of every batch item, then bfs_cluster (bfs_cluster.cpp:60-86).
-    prob: the softmax of the semantic scores (:422) as float32 [N, C]. info: see _note."""
+    prob: the softmax of the semantic scores (:422) as float32 [N, C]. info: see _note; also 'neighbours', the sum of
+    the ball query's list lengths over all classes."""
     g, tc = cfg['grouping_cfg'], cfg['test_cfg']
     mean = np.asarray(g['class_numpoint_mean'], np.float32)
     batch_idxs = np.asarray(batch_idxs, np.int32)
@@ -137,7 +138,10 @@ def grouping(prob, pt_offsets, batch_idxs, coords_float, cfg, batch_size, info=N
         b = batch_idxs[obj]
         xyz = (coords_float[obj] + pt_offsets[obj]).astype(np.float32)  # :452, float32 like the tensors
         nidx, sl = oracle.ballquery_batch_p_grid(xyz, b, _batch_offsets(b, batch_size), g['radius'])
+        if info is not None:
+            info['neighbours'] = info.get('neighbours', 0) + nidx.size
         pidx, poff = oracle.bfs_cluster(mean, nidx, sl, g['npoint_thr'], c)
+        del nidx  # up to 1000 entries per point: freed before the next class's lists
         pidx[:, 1] = obj[pidx[:, 1]]  # :464
         _note(info, c, poff)
         _append(idx_list, off_list, pidx, poff)

@@ -1,7 +1,8 @@
 """Generate the fixtures that pin this repo's host-side model logic on the UNMODIFIED reference SoftGroup code:
 
-  * tests/golden/ref_model_meta.json -- the `model` sections of the reference configs/*.yaml files and the reference
-    SoftGroup(scannet) state_dict names and shapes (in order);
+  * tests/golden/ref_model_meta.json -- the `model` sections of the reference configs this repo restates (`configs`,
+    by configs.CONFIGS name), the `model` section of every configs/**/*.yaml the reference ships (`yamls`, by path) and
+    the reference SoftGroup(scannet) state_dict names and shapes (in order);
   * tests/golden/ref_host_methods.npz -- what the reference's own CUDA-free methods return on the inputs of
     tests/test_host_vs_reference_methods.py and tests/test_host_grouping.py (panoptic_fusion, get_gt_instances,
     merge_4_parts, get_level, pyramid_inverse_map, forward_grouping with oracle stand-ins for its device ops).
@@ -12,6 +13,7 @@ Needs a checkout of the reference (thangvubk/SoftGroup) and runs on the CPU:
 
 The tests read only the fixtures; --check regenerates them in memory and compares with the stored files.
 """
+import glob
 import importlib
 import json
 import os
@@ -30,7 +32,9 @@ YAMLS = {'scannet': 'configs/softgroup/softgroup_scannet.yaml',
          's3dis': 'configs/softgroup/softgroup_s3dis_fold5.yaml',
          'kitti': 'configs/softgroup/softgroup_kitti.yaml',
          'stpls3d++': 'configs/softgroup++/softgroup++_stpls3d.yaml',
-         'scannet++': 'configs/softgroup++/softgroup++_scannet.yaml'}
+         'scannet++': 'configs/softgroup++/softgroup++_scannet.yaml',
+         's3dis++': 'configs/softgroup++/softgroup++_s3dis_fold5.yaml',
+         'stpls3d': 'configs/softgroup/softgroup_stpls3d.yaml'}
 
 
 def import_reference_model(ref_root):
@@ -56,6 +60,9 @@ def make(ref_root):
 
     ref_module = import_reference_model(ref_root)
     meta = dict(configs={k: yaml.safe_load(open(os.path.join(ref_root, p)))['model'] for k, p in YAMLS.items()})
+    paths = sorted(os.path.relpath(p, ref_root) for p in glob.glob(os.path.join(ref_root, 'configs', '**', '*.yaml'),
+                                                                   recursive=True))
+    meta['yamls'] = {p: yaml.safe_load(open(os.path.join(ref_root, p)))['model'] for p in paths}
     sd = ref_module.SoftGroup(**model_cfg('scannet')).state_dict()
     meta['state_dict_scannet'] = [[k, list(v.shape)] for k, v in sd.items()]
 

@@ -27,6 +27,7 @@ from seeded_weights import CFG_OVERRIDES, SCAN, WEIGHT_SEED, fill_seeded, load_c
 from softgroup_b200 import synth  # noqa: E402
 from softgroup_b200.configs import model_cfg  # noqa: E402
 from softgroup_b200.model import SoftGroup  # noqa: E402
+from softgroup_b200.ops.functions import BALLQUERY_MAX_CAPACITY  # noqa: E402
 
 REL = 2e-4  # the fixture's float bar (tests/test_gpu_forward_golden.py), relative to the largest golden magnitude
 
@@ -185,7 +186,10 @@ def test_workload_cases_follow_bench():
 def test_config_cases_reach_their_paths():
     """The table of forward_cases.CONFIG_CASES, from the injection alone (its float32 softmax on the CPU): pp_lvlfusion
     groups every class at pyramid level 1 from voxel rows, pp_lvlfusion_l2 one class holding every thing voxel at level
-    2, scannet200 at least 20 classes, c5_level3 one class of 1.25M points at level 3."""
+    2, scannet200 at least 20 classes, c5_level3 one class of 1.25M points at level 3, s3dis_pp the whole S3DIS room as
+    voxel rows with one merged class at level 2 and nine at level 1, stpls3d the 1.5M-point tile through one ball query
+    whose lists hold more than 1e9 neighbours (4.95 GB, past 4 GiB of byte offset) yet fit one int32 cursor. The
+    stpls3d neighbour total is counted with the grid ball query of the restatement (about a minute)."""
     for case in fc.CONFIG_CASES:
         w = fc.build_config_case(case)
         cfg, scan, counts = w['cfg'], w['scan'], w['counts']
@@ -205,9 +209,28 @@ def test_config_cases_reach_their_paths():
         elif case.name == 'scannet200':
             assert not cfg['grouping_cfg'].get('with_pyramid') and cfg['semantic_classes'] == 200
             assert cfg['instance_classes'] == 198 and np.unique(sem[inst >= 0]).size >= 20
-        else:
-            assert case.name == 'c5_level3' and levels == {9: 3}
+        elif case.name == 'c5_level3':
+            assert levels == {9: 3}
             assert (inst >= 0).sum() == counts[9] == 1250073
+        elif case.name == 's3dis_pp':  # thing points of class 7 merged into class 5
+            assert not cfg['test_cfg']['x4_split'] and cfg['sem2ins_classes'] == [0, 1]
+            assert scan['coords'].shape[0] == 800000 and w['inj'][0].shape[0] == 687804 and thing_voxels == 576809
+            assert 7 not in counts and counts[5] == 181026 and sum(counts.values()) == 579163
+            assert levels[5] == 2 and sorted(c for c, lv in levels.items() if lv == 1) == [2, 3, 4, 6, 8, 9, 10, 11, 12]
+        else:
+            assert case.name == 'stpls3d' and not cfg['grouping_cfg'].get('with_pyramid') and case.relabel is None
+            assert scan['coords'].shape[0] == 1500000 and len(counts) == 14
+            n_sel = sum(counts.values())
+            assert n_sel == 1250088 and n_sel * 1000 <= BALLQUERY_MAX_CAPACITY
+            prob = torch.from_numpy(w['inj'][0]).softmax(-1).numpy()
+            g = cfg['grouping_cfg']
+            total = 0
+            for c in counts:
+                obj = np.flatnonzero(prob[:, c] > np.float32(g['score_thr']))
+                xyz = (scan['coords_float'][obj] + w['inj'][1][obj]).astype(np.float32)
+                total += oracle.ballquery_total_grid(xyz, np.zeros(obj.size, np.int32), np.array([0, obj.size], np.int32),
+                                                     g['radius'])
+            assert total == 1237543570 and total * 4 > 4 << 30
 
 
 @pytest.mark.parametrize('lvl_fusion', [False, True])

@@ -10,7 +10,10 @@ dataloader's collated batch). Its result dict is compared with
     own forward_test on CPU stand-ins).
 
 The `scannet++` case runs the reference's own lvl_fusion / pyramid / octree code path (softgroup.py:309-312, 332-334,
-427-463, 560-561) on the GPU ops -- the reference-order procedure for this repo's sparse lvl_fusion implementation."""
+427-463, 560-561) on the GPU ops -- the reference-order procedure for this repo's sparse lvl_fusion implementation.
+`s3dis++` runs it with sem2ins classes: their instances are the per-point class masks taken through v2p_map
+(:556-561). `stpls3d` runs the plain one-pass grouping with mean_active 3, so the reference's ball query regrows its
+buffer (functions.py:258-265) on the shim's ballquery_batch_p."""
 import os
 import sys
 
@@ -19,7 +22,7 @@ import pytest
 import torch
 
 from softgroup_b200 import harness, synth
-from softgroup_b200.configs import model_cfg
+from softgroup_b200.configs import SHAPE_OF, model_cfg
 from softgroup_b200.model import SoftGroup
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -109,17 +112,31 @@ def test_reference_class_runs_on_b200_and_matches(ref_module):
     assert np.abs(conf - gold['inst_conf']).max() <= 2e-4 * max(1.0, np.abs(gold['inst_conf']).max())
 
 
-@pytest.mark.parametrize('name,n_points', [('scannet', 30000), ('scannet++', 20000)])
+# grouping thresholds that give proposals on a random-weight (calibrated-head) model: the yaml values (thresholds relative
+# to the real datasets' class sizes) select nothing there -- both models returned 0 instances
+GROUPING_OVERRIDES = {
+    'scannet': (dict(radius=0.15, class_numpoint_mean=[-1.] * 20, npoint_thr=100), dict(min_npoint=50)),
+    'scannet++': (dict(radius=0.15, class_numpoint_mean=[-1.] * 20, npoint_thr=100), dict(min_npoint=50)),
+    's3dis++': (dict(radius=0.15, class_numpoint_mean=[-1.] * 13, npoint_thr=20), dict(min_npoint=20)),
+    'stpls3d': (dict(radius=1.5, class_numpoint_mean=[-1.] * 15, npoint_thr=5), dict(min_npoint=5)),
+}
+
+
+@pytest.mark.parametrize('name,n_points', [('scannet', 30000), ('scannet++', 20000), ('s3dis++', 20000),
+                                           ('stpls3d', 20000)])
 def test_reference_class_vs_restructured_forward(ref_module, name, n_points):
-    """Full-size model (32 channels x 7 levels); 'scannet++' = pyramid + octree + lvl_fusion at test time."""
-    # grouping thresholds that give proposals on a random-weight (calibrated-head) model: the yaml values (4 cm radius,
-    # thresholds relative to ScanNet class sizes) select nothing there -- both models returned 0 instances
-    cfg = model_cfg(name, grouping_cfg=dict(radius=0.15, class_numpoint_mean=[-1.] * 20, npoint_thr=100),
-                    test_cfg=dict(min_npoint=50))
-    scan = synth.make_scan('c2_scannet', seed=5, n_points=n_points)
+    """Full-size model (7 levels) on a scan of the config's own shape; 'scannet++' and 's3dis++' = pyramid + octree +
+    lvl_fusion at test time, 's3dis++' with sem2ins classes, 'stpls3d' = one-pass grouping at mean_active 3."""
+    grouping, test = GROUPING_OVERRIDES[name]
+    cfg = model_cfg(name, grouping_cfg=grouping, test_cfg=test)
+    scan = synth.make_scan(SHAPE_OF[name], seed=5, n_points=n_points)
     ours, ref = _pair(ref_module, cfg, scan=scan)
     batch = harness.collate_like_reference(scan)
     with torch.no_grad():
         r_ref = ref(dict(batch))
         r_our = ours(dict(batch))
     _compare(r_ref, r_our, n_points)
+    if cfg['sem2ins_classes']:
+        labels = [int(x['label_id']) for x in r_ref['pred_instances']]
+        assert set(labels) & {i + 1 for i in cfg['sem2ins_classes']}, labels
+        assert set(labels) - {i + 1 for i in cfg['sem2ins_classes']}, labels

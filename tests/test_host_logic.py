@@ -81,32 +81,66 @@ def test_rle_encode_many_empty():
 
 # ---- configs are restated data: pin them on the reference YAMLs (their `model` sections are stored in
 #      tests/golden/ref_model_meta.json by tests/golden/make_reference_golden.py) ---------------------------------------
+def _ref_model_meta():
+    import json
+    return json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_model_meta.json')))
+
+
+def _config_differences(ours, ref):
+    """The keys of a reference `model` section that a restated config (model_cfg kwargs) does not equal: the model's
+    shape, grouping_cfg, instance_voxel_cfg and test_cfg. fixed_modules, semantic_weight and train_cfg matter only in
+    training."""
+    diff = [k for k in ('channels', 'num_blocks', 'semantic_classes', 'instance_classes', 'sem2ins_classes',
+                        'semantic_only', 'ignore_label') if ours[k] != ref[k]]
+    diff += [k for k in ('in_channels', 'with_coords') if k in ref and ours.get(k) != ref[k]]
+    for sec in ('grouping_cfg', 'instance_voxel_cfg', 'test_cfg'):
+        for key, val in ref[sec].items():
+            got = ours[sec].get(key)
+            if key == 'class_numpoint_mean' and isinstance(got, list):  # YAML ints and floats are the same numbers
+                same = [float(v) for v in got] == [float(v) for v in val]
+            else:
+                same = key in ours[sec] and got == val
+            if not same:
+                diff.append('%s.%s' % (sec, key))
+    return diff
+
+
 @pytest.mark.parametrize('name,path', [('scannet', 'configs/softgroup/softgroup_scannet.yaml'),
                                        ('s3dis', 'configs/softgroup/softgroup_s3dis_fold5.yaml'),
                                        ('kitti', 'configs/softgroup/softgroup_kitti.yaml'),
                                        ('stpls3d++', 'configs/softgroup++/softgroup++_stpls3d.yaml'),
-                                       ('scannet++', 'configs/softgroup++/softgroup++_scannet.yaml')])
+                                       ('scannet++', 'configs/softgroup++/softgroup++_scannet.yaml'),
+                                       ('s3dis++', 'configs/softgroup++/softgroup++_s3dis_fold5.yaml'),
+                                       ('stpls3d', 'configs/softgroup/softgroup_stpls3d.yaml')])
 def test_configs_match_reference_yaml(name, path):
-    import json
-    meta = json.load(open(os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ref_model_meta.json')))
+    meta = _ref_model_meta()
     ref = meta['configs'][name]
-    ours = configs.model_cfg(name)
-    for key in ('channels', 'num_blocks', 'semantic_classes', 'instance_classes', 'sem2ins_classes', 'semantic_only',
-                'ignore_label'):
-        assert ours[key] == ref[key], key
-    for key in ('in_channels', 'with_coords'):
-        if key in ref:
-            assert ours[key] == ref[key], key
-    for key, val in ref['grouping_cfg'].items():
-        got = ours['grouping_cfg'][key]
-        if isinstance(val, list):
-            assert [float(v) for v in got] == [float(v) for v in val], key
+    assert meta['yamls'][path] == ref
+    assert _config_differences(configs.model_cfg(name), ref) == []
+
+
+def test_every_reference_yaml_is_restated_or_semantic_only():
+    """Every config the reference ships (the `model` section of each configs/**/*.yaml) either equals a restated config
+    of configs.CONFIGS on the keys inference reads, or is a semantic_only backbone config evaluated on 'semantic' alone:
+    its forward_test stops after the point-wise heads (no grouping, no instances), which the restated configs run
+    stage by stage, so it needs no restatement of its own. A config the reference adds fails here until it is
+    restated or shown to be such a backbone config."""
+    yamls = _ref_model_meta()['yamls']
+    assert len(yamls) == 23
+    backbone_only, restated = [], {}
+    for path, ref in sorted(yamls.items()):
+        same = [n for n in configs.CONFIGS if not _config_differences(configs.model_cfg(n), ref)]
+        if same:
+            restated[path] = same
         else:
-            assert got == val, key
-    for key, val in ref['instance_voxel_cfg'].items():
-        assert ours['instance_voxel_cfg'][key] == val, key
-    for key, val in ref['test_cfg'].items():
-        assert ours['test_cfg'][key] == val, key
+            assert ref['semantic_only'] and set(ref['test_cfg'].get('eval_tasks', [])) <= {'semantic'}, path
+            backbone_only.append(path)
+    # eleven backbone files, six distinct sections (the SoftGroup++ S3DIS folds again share one)
+    assert len(backbone_only) == 11 and all('_backbone' in p for p in backbone_only)
+    assert len({repr(sorted(yamls[p].items())) for p in backbone_only}) == 6
+    # the six S3DIS folds of SoftGroup++ share one model section
+    assert all(restated['configs/softgroup++/softgroup++_s3dis_fold%d.yaml' % k] == ['s3dis++'] for k in range(1, 7))
+    assert sorted(set(sum(restated.values(), []))) == sorted(set(configs.CONFIGS) - {'scannet200'})
 
 
 # ---- BatchNorm1d(eval) folding (softgroup.py:54, eps = 1e-4) ---------------------------------------------------
